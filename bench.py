@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Benchmark of the ODISE inference hot path on B200 (contract: see the task brief / DESIGN.md §5).
+"""Benchmark of the ODISE inference hot path on an H100 (DESIGN.md §5).
 
     python bench.py --gpus N --steps K --warmup W                 # our arm (one rank per GPU under torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path (oracle), rank 0 only
     python bench.py --config c3|c4|c5 ...                          # the other BASELINE.json configs (c2 = default)
+    python bench.py ... --dump-outputs DIR                         # + what the timed step computed, as DIR/<name>.npy
 
 A step = one pass of the per-image pipeline over a batch of synthetic images: CLIP ViT-L/14-336 image tower on every
 512^2 crop + KL-VAE encoder / truncated decoder taps [unless --hot-path-only] -> implicit captioner -> UNet feature
@@ -13,7 +14,7 @@ ensemble -> semantic + panoptic + instance inference at the input resolution (od
 ODISEEngine.infer(outputs="panoptic") with pinned-host uint8 images in and the panoptic map + segment table + instance
 table + class logits out.
 
-BASELINE.json configs:  c2 (default) 1xB200, batch 4 x 1024^2, ADE-150 | c3 image-sharded 8xB200, COCO-133 |
+BASELINE.json configs:  c2 (default) 1 GPU, batch 4 x 1024^2, ADE-150 | c3 image-sharded over N GPUs, COCO-133 |
 c4 MSDeformAttn + masked-attention decoder microbench (256 queries x 4 scales, HBM GB/s) | c5 ADE-847 (1342 prompts) at
 1280^2 (9 overlapping crops per image), reporting the mask-embed x text GEMM TFLOP/s.
 """
@@ -61,10 +62,15 @@ def parse():
                          "(not a parity mode)")
     ap.add_argument("--vocab", default=None, choices=sorted(VOCABS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (float32 / "
+                         "float64, a fixed seeded sample of the larger ones, 64 MB in all)")
     ap.add_argument("--hot-path-only", action="store_true",
                     help="skip the KL-VAE (SURVEY.md 8f-1) and CLIP image tower (8f-2) stages: their taps / latent / "
                          "image embedding enter as synthetic tensors")
     a = ap.parse_args()
+    if a.dump_outputs and (a.config == "c4" or a.impl == "reference"):
+        ap.error("--dump-outputs writes the outputs of the pipeline step: not available with --config c4 or --impl reference")
     c = CONFIGS[a.config]
     a.batch = a.batch or c["batch"]
     a.size = a.size or c["size"]
@@ -78,7 +84,8 @@ def peaks():
         d = json.load(open(p))
         return dict(bf16_burst=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     hbm=d["hbm_gbs"], source="measured")
-    return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback")
+    # NVIDIA's data sheet for the H100 SXM (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s; a ceiling, not a measurement
+    return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm=3350.0, source="H100 SXM data sheet")
 
 
 def n_crops(size):
@@ -87,7 +94,7 @@ def n_crops(size):
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region (SM clock and throttle reasons next to the result)."""
 
     def __init__(self, index):
         self.index = index
@@ -218,15 +225,12 @@ def run_reference(args):
                           "own CUDA kernel, oracle/_ref) is reported inside the c4 line of the `ours` arm"}), flush=True)
         return
     cpu = CpuHotPath(args.size, args.vocab, full=args.full)
-    t_start = time.perf_counter()
     for _ in range(min(args.warmup, 1)):
         cpu.sample()
     vals, info = [], None
     for _ in range(args.steps):
         info = cpu.sample()
         vals.append(info["value"])
-        if time.perf_counter() - t_start > 200:                 # keep the arm within a few minutes
-            break
     v = statistics.mean(vals)
     info["value"] = v
     ncls, npr = VOCABS[args.vocab]
@@ -259,7 +263,7 @@ def run_c4(args, dev):
     """BASELINE.json configs[3]: MSDeformAttn sampling + masked-attention decoder, 256 queries x 4 scales, HBM GB/s.
     (a) the deformable-attention op on the 4-level pyramid of a 1024^2 input (strides 8..64), N = batch images, once with
     every pixel a query (pixel-decoder encoder, Lq = S) and once with 256 queries; ours (reference ABI and fused-front
-    variants) next to the REFERENCE's own CUDA kernel compiled for sm_100a (oracle/_ref);
+    variants) next to the REFERENCE's own CUDA kernel compiled for sm_90a (oracle/_ref, when it was built);
     (b) the 9-layer masked-attention decoder + 10 prediction heads with 256 queries cycling over 4 scales."""
     from odise_b200 import lib, ops, spec
     from odise_b200.head import HeadEngine
@@ -292,8 +296,8 @@ def run_c4(args, dev):
         def ours_fused():
             ops.msda_fused(value, dss, dls, dref, doffs, dlog, N, S, M, D, L, Lq, P, want_f32=False)
 
-        reps = 20 if Lq == S else 200
-        t_abi, t_fused = _time_ms(ours_abi, reps), _time_ms(ours_fused, reps)
+        reps = args.steps
+        t_abi, t_fused = _time_ms(ours_abi, reps, args.warmup), _time_ms(ours_fused, reps, args.warmup)
         # what the gathers move through L1: 4 corners x 128 B per (query, head, sample)
         l1_bytes = 128.0 * 4 * N * Lq * M * L * P
         # compulsory bytes (SURVEY.md §8d): value once (at most what the samples can touch) + loc / attn (3 floats per
@@ -306,7 +310,7 @@ def run_c4(args, dev):
             from oracle import refmsda
             if refmsda.available():
                 ro = torch.empty_like(out)
-                t_ref = _time_ms(lambda: refmsda.forward(value, dss, dls, loc, aw, 128, out=ro), reps)
+                t_ref = _time_ms(lambda: refmsda.forward(value, dss, dls, loc, aw, 128, out=ro), reps, args.warmup)
                 ours_abi()
                 torch.cuda.synchronize()
                 r.update(reference_kernel_us=1e3 * t_ref, reference_kernel_gbs=nbytes / t_ref / 1e6,
@@ -326,7 +330,7 @@ def run_c4(args, dev):
     c0 = lib.launch_count()
     he.transformer_decoder(pd, N)
     launches = lib.launch_count() - c0
-    t_dec = _time_ms(lambda: he.transformer_decoder(pd, N), 10)
+    t_dec = _time_ms(lambda: he.transformer_decoder(pd, N), args.steps, args.warmup)
     HW = (args.size // 4) ** 2
     plane = 4.0                                     # bytes per element of a (hi, lo) bf16 operand pair
     # K and V^T planes (head-padded 8 x 64 columns) of every layer, read once by its cross-attention
@@ -342,12 +346,12 @@ def run_c4(args, dev):
     enc = res["encoder_Lq=S"]
     line = {
         "metric": "MSDeformAttn + masked-attention decoder microbench, 256 queries x 4 scales, HBM GB/s",
-        "value": enc["ours_abi_gbs"], "unit": "GB/s", "n_gpus": 1, "steps": 20, "warmup": 3,
+        "value": enc["ours_abi_gbs"], "unit": "GB/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": enc["ours_abi_us"] / 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"c4: MSDeformAttn forward, N={N}, 4 levels {shapes}, S={S}, M=8, D=32, P=4 (value = compulsory "
                                "bytes / time of odise_msda_forward_f32 with Lq = S); masked-attention decoder Q=256 x 4 scales",
-                   "l2": "value (N x 22 MB) + loc/attn/out streams > 126 MB L2 at N = 4"},
+                   "l2": "value (N x 22 MB) + loc/attn/out streams > 50 MB L2 at N = 4"},
         "roofline": {"bound": "hbm", "kernel": "msda_d32_kernel", "achieved": enc["ours_abi_gbs"], "peak": pk["hbm"],
                      "unit": "GB/s", "frac": enc["ours_abi_gbs"] / pk["hbm"], "traffic": None,
                      "note": "the gathers move 4 corners x 128 B per (query, head, sample) through L1: "
@@ -359,6 +363,36 @@ def run_c4(args, dev):
 
 
 # ----------------------------------------------------------------------------------------------- our arm
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out, directory):
+    """The arrays a caller of the timed step receives (its result dict; `aux` = the intermediate heads is left out), as
+    <directory>/<name>.npy in float32 (float64 stays float64).  Arrays too large for an equal share of DUMP_BYTES are
+    replaced by a fixed, seeded sample of their flattened elements (the same indices for every build)."""
+    import numpy as np
+    flat = []
+
+    def walk(prefix, v):
+        if torch.is_tensor(v):
+            flat.append((prefix, v))
+        elif isinstance(v, dict):
+            for k in sorted(v):
+                if k != "aux":
+                    walk(f"{prefix}.{k}" if prefix else k, v[k])
+    walk("", out)
+    torch.cuda.synchronize()
+    cap = DUMP_BYTES // (8 * max(1, len(flat)))          # elements per array (8 bytes: the float64 worst case)
+    os.makedirs(directory, exist_ok=True)
+    for name, t in flat:
+        t = t.detach().reshape(-1)
+        if t.numel() > cap:
+            idx = torch.randint(0, t.numel(), (cap,), generator=torch.Generator().manual_seed(0)).sort().values
+            t = t[idx.to(t.device)]
+        a = t.cpu().to(torch.float64 if t.dtype == torch.float64 else torch.float32).numpy()
+        np.save(os.path.join(directory, f"{name}.npy"), a)
+
+
 def main():
     args = parse()
     args.full = not args.hot_path_only
@@ -431,6 +465,8 @@ def main():
     if rank == 0:
         sampler.start()
     ms_dev = timed(dev_step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     for _ in range(max(1, args.warmup // 2)):
         e2e_step()
     ms_e2e = timed(e2e_step, args.steps)
@@ -478,8 +514,7 @@ def main():
             t2 = _time_ms(lambda: lib.gemm(ce_p, cv["te_p"], nmma=nmma, alpha=100.0, out=sims2), 200)
             extra["clip_match_gemm"]["maskclip_head"] = {"M": B * eng.Q, "N": v["Kp"], "K": 768, "us": 1e3 * t2,
                                                          "tflops": 2.0 * B * eng.Q * v["Kp"] * 768 / t2 / 1e9}
-        extra["clip_match_gemm"]["note"] = ("400 x 1342 outputs: one wave of 128 x 128 tiles, launch / pipeline-fill bound "
-                                            "(~10 us); the same GEMM at 6400 rows runs at > 130 TFLOP/s (profiles/ncu_r1)")
+        extra["clip_match_gemm"]["note"] = "400 x 1342 outputs: one wave of 128-row tiles, launch / pipeline-fill bound"
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -488,15 +523,6 @@ def main():
     ips = world * B * args.steps / (ms_dev / 1000.0)
     ips_e2e = world * B * args.steps / (ms_e2e / 1000.0)
     achieved = gemm_flops / (gemm_ms / 1000.0) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-    traffic_src = None
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-        except Exception:
-            traffic = None
     metric = METRIC if S == 1024 else METRIC.replace("1024x1024", f"{S}x{S}")
     line = {
         "metric": metric, "value": ips, "unit": "images/s", "n_gpus": world, "steps": args.steps,
@@ -517,7 +543,7 @@ def main():
                                    "tensors (SURVEY.md §8f rows f-1/f-2)"),
                    "weights": "random-init (seed 0), SD-v1 / ODISE shapes", "global_batch": world * B,
                    "parallelism": f"dp{world} (image sharded)", "precision_mode": args.precision,
-                   "l2": "working set >> 126 MB L2: ~3.6 GB of weight planes + multi-GB activations stream every step",
+                   "l2": "working set >> 50 MB L2: ~3.6 GB of weight planes + multi-GB activations stream every step",
                    "cuda_graph": True},
         "e2e": {"value": ips_e2e, "unit": "images/s", "h2d_bytes_per_step": int(images.numel()),
                 "d2h_bytes_per_step": eng.d2h_bytes(), "ms_per_step": ms_e2e / args.steps,
@@ -525,17 +551,16 @@ def main():
         "gpu_launches": int(launches_per_step * args.steps * 2),
         "gpu_launches_per_step": int(launches_per_step),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 GEMM / implicit conv, all launches of a step)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel (wgmma GEMM / implicit conv, all launches of a step)",
                      "achieved": achieved, "peak": pk["bf16_sustained"], "unit": "TFLOP/s",
-                     "frac": achieved / pk["bf16_sustained"], "peak_source": pk["source"] + " sustained cuBLAS bf16",
+                     "frac": achieved / pk["bf16_sustained"], "peak_source": pk["source"],
                      "launches": int(n_gemm), "gemm_ms_per_step": gemm_ms, "algorithmic_tflop_per_step": gemm_flops / 1e12,
-                     "mma_kind": "tcgen05.mma kind::f16 (bf16 in, fp32 TMEM accumulate)" +
+                     "mma_kind": "wgmma.mma_async bf16 (fp32 register accumulate)" +
                                  (", 3 MMAs per k-step (bf16x3 split)" if nmma == 3 else "") +
-                                 (" for the head; VAE / CLIP / UNet / projections: kind::f16 (fp16 hi x hi) + kind::f8f6f4 "
-                                  "(e5m2 cross terms, K = 32) = 2 MMA units per k-step" if nmma == 2 else ""),
+                                 (" for the head; VAE / CLIP / UNet / projections: fp16 k16 (hi x hi) + e5m2 k32 "
+                                  "(cross terms) = 2 MMA units per k-step" if nmma == 2 else ""),
                      "tensor_pipe_equiv_frac": achieved * nmma / pk["bf16_sustained"],
-                     "unet_frac_of_step": (UNET_TFLOP_PER_CROP * crops * B) / (gemm_flops / 1e12), "traffic": traffic,
-                     "traffic_source": traffic_src,
+                     "unet_frac_of_step": (UNET_TFLOP_PER_CROP * crops * B) / (gemm_flops / 1e12),
                      "unet_feature_pass": {
                          "ms": unet_ms, "crops": nc_all, "algorithmic_tflop": UNET_TFLOP_PER_CROP * nc_all,
                          "achieved_tflops": UNET_TFLOP_PER_CROP * nc_all / (unet_ms / 1000.0),

@@ -1,4 +1,4 @@
-/* odise_b200 C ABI — the drop-in boundary for the ODISE per-image inference hot path on B200 (sm_100a).
+/* odise_b200 C ABI — the drop-in boundary for the ODISE per-image inference hot path on H100 (sm_90a).
  *
  * Plain pointers and sizes only; the caller owns every buffer; every entry point is asynchronous on the CUDA
  * stream it is given (cudaStream_t passed as void*) and returns 0 or an error code (ODISE_ERR_* or a cudaError_t).
@@ -78,7 +78,7 @@ int odise_msda_fused_f32(const float* value, const int64_t* spatial_shapes, cons
                          void* out_hi, void* out_lo, int N, int S, int M, int D, int L, int Lq, int P, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * tcgen05 GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
+ * wgmma GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
  * Replaces F.conv2d / F.linear / torch.einsum call sites of the path (ldm ResBlock & attention linears via
  * odise/modeling/meta_arch/ldm.py:469-491; M2F linears; odise.py:746 mask einsum; odise.py:955-959 pooling;
  * odise.py:192-205 CLIP match).
@@ -120,7 +120,7 @@ typedef struct odise_gemm_desc {
 } odise_gemm_desc;
 int odise_gemm_bf16(const odise_gemm_desc* desc, void* stream);
 /* Host-only: the cost-model tile choice of odise_gemm_bf16 for a problem — output-tile width *bn (64 | 128 | 160 | 256) and
- * *pair = 1 when CTA pairs run 2-SM MMAs (tcgen05 cta_group::2; BN = 256, K >= 1024, M tiles that pair up).  It is what the
+ * *pair (always 0: the sm_90a kernel does not pair CTAs; F16Q8 (nmma 2) uses BN <= 128).  It is what the
  * GEMM uses under CUDA-graph capture / with ODISE_GEMM_AUTOTUNE=0 and the first candidate of the one-time per-shape autotune. */
 int odise_gemm_tile_policy(int M, int N, int K, int batch, int conv3x3, int nmma, int* bn, int* pair);
 /* optional per-launch timing of odise_gemm_bf16 (CUDA events on the launch stream; not for use under graph capture):
@@ -239,7 +239,7 @@ int odise_nchw_to_nhwc_f32(const float* src, float* dst, long long ldd, int B, i
 int odise_nhwc_to_nchw_f32(const float* src, long long lds, float* dst, int B, int C, int HW, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Fused flash attention on tcgen05 (UNet SpatialTransformer self- and cross-attention; ldm CrossAttention,
+ * Fused flash attention on wgmma (UNet SpatialTransformer self- and cross-attention; ldm CrossAttention,
  * SURVEY.md App. A): out[b, t, h*d + j] = softmax_k(scale * q.k) v.
  * Operands are HEAD-PADDED (hi, lo) planes: head h occupies columns [h*HS, h*HS + d) with HS = 64 (d <= 64),
  * 128 (d <= 80) or 192 (d == 160: the 16x16 / 8x8 UNet levels), pad columns zero:  q [B*Tq, heads*HS] (ldq), k [B*tk_stride, heads*HS] (ldk), and V TRANSPOSED
@@ -249,7 +249,7 @@ int odise_nhwc_to_nchw_f32(const float* src, long long lds, float* dst, int B, i
  * d <= 80, or d == 160 (other head sizes: odise_gemm_bf16 + odise_softmax_split_f32, e.g. the VAE mid block's d = 512).
  * nmma = 3: q, k are bf16 (hi, lo) planes, vt is an **fp16** (hi, lo) pair (odise_gemm_desc.out_planes_fp16 /
  * odise_split_f16_f32): S = Q K^T runs hi*hi + hi*lo + lo*hi, the probabilities are rounded once to fp16 and
- * O = P16 V_hi + P16 V_lo (tcgen05 kind::f16 needs A and B of one 16-bit type).  nmma = 1: bf16 hi planes only.
+ * O = P16 V_hi + P16 V_lo (wgmma needs A and B of one 16-bit type).  nmma = 1: bf16 hi planes only.
  * out fp32 and/or (hi, lo) bf16 planes, UNPADDED [B*Tq, heads*d] with row stride ldo.
  * mask_bits / row_any (optional, from odise_attn_mask_bits_f32): the Mask2Former decoder's masked cross-attention
  * (d = 32) on the same tensor-core kernel — key k of row (b, t) is dropped when its bit is 0 and row_any != 0. */

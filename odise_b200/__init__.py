@@ -1,6 +1,6 @@
-"""odise_b200: B200-native (sm_100a) engine for the ODISE open-vocabulary panoptic inference hot path.
+"""odise_b200: H100-native (sm_90a) engine for the ODISE open-vocabulary panoptic inference hot path.
 
 Host side is Python (like the reference); all device arithmetic lives in libodise_b200.so (include/odise_b200.h),
-hand-written CUDA for sm_100a: tcgen05/TMEM/TMA GEMM + implicit conv, tcgen05 flash attention, warp-shuffle
+hand-written CUDA for sm_90a: wgmma/TMA GEMM + implicit conv, wgmma flash attention, warp-shuffle
 deformable / masked attention, fused elementwise passes.  No CPU or eager fallback exists."""
 __version__ = "0.1.0"

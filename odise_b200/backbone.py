@@ -1,4 +1,4 @@
-"""B200 engine for ODISE's diffusion backbone glue (SURVEY.md §8a rows a2-a6): the sliding 512x512 crops of
+"""H100 engine for ODISE's diffusion backbone glue (SURVEY.md §8a rows a2-a6): the sliding 512x512 crops of
 FeatureExtractorBackbone.slide_forward (odise/modeling/backbone/feature_extractor.py:181-250), the implicit
 captioner front of LdmImplicitCaptionerExtractor.forward (odise/modeling/meta_arch/ldm.py:697-718), q_sample at
 t = 0 (odise/modeling/diffusion/gaussian_diffusion.py:275-292) with the reference's shared noise (ldm.py:271-277),

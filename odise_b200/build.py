@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libodise_b200.so (sm_100a only) and of the C oracle.
+"""In-tree nvcc build of libodise_b200.so (sm_90a only) and of the C oracle.
 
 Used by __graft_entry__.build(); no torch extension machinery: the product is a plain C-ABI shared library
 (include/odise_b200.h) loaded with ctypes."""
@@ -12,7 +12,7 @@ CSRC = os.path.join(ROOT, "odise_b200", "csrc")
 OUT = os.path.join(ROOT, "odise_b200", "libodise_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include"), "-I", CSRC,
     "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]

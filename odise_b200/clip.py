@@ -1,9 +1,9 @@
-"""B200 engine for the CLIP ViT-L/14-336 image tower behind ClipAdapter.embed_image (SURVEY.md §8f-2;
+"""H100 engine for the CLIP ViT-L/14-336 image tower behind ClipAdapter.embed_image (SURVEY.md §8f-2;
 odise/modeling/meta_arch/clip.py:177-231, called from LdmImplicitCaptionerExtractor.forward, ldm.py:705).
 
 crop [B, 3, 512, 512] in [0,1] -> bicubic 336 + CLIP normalisation (odise_clip_preprocess) -> 14x14 patch embedding as a
-GEMM -> 24 pre-LN transformer blocks (QKV / out / MLP on the tcgen05 GEMM with fused bias, QuickGELU and residual
-epilogues; attention on the tcgen05 flash kernel, d = 64) -> ln_post + projection of the class token -> [B, 768].
+GEMM -> 24 pre-LN transformer blocks (QKV / out / MLP on the wgmma GEMM with fused bias, QuickGELU and residual
+epilogues; attention on the wgmma flash kernel, d = 64) -> ln_post + projection of the class token -> [B, 768].
 Tokens per image are padded 577 -> 584 rows so every TMA box start stays 16-byte aligned; pad keys are masked.
 """
 import torch

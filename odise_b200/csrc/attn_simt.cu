@@ -1,4 +1,4 @@
-// Warp-shuffle attention kernels of the Mask2Former transformer decoder (SURVEY.md §8a rows b7-b9), sm_100a.
+// Warp-shuffle attention kernels of the Mask2Former transformer decoder (SURVEY.md §8a rows b7-b9), sm_90a.
 //
 // Reference: nn.MultiheadAttention(256, 8) inside CrossAttentionLayer / SelfAttentionLayer
 // (mask2former_transformer_decoder.py:22,80,98-110,40-50) fed a materialised bool attn_mask [B*8, Q, HW] that

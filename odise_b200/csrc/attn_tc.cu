@@ -1,24 +1,20 @@
-// Fused flash attention on tcgen05 for the SD-v1 UNet SpatialTransformer (SURVEY.md §8a row a7.2): self-attention
+// Fused flash attention on wgmma for the SD-v1 UNet SpatialTransformer (SURVEY.md §8a row a7.2): self-attention
 // (4096 / 1024 tokens, head dim 40 / 80) and cross-attention over the 77-token context.  Reference: ldm
 // CrossAttention = softmax(q k^T * d^-0.5) v via einsum or xformers (un-vendored; call sites ldm.py:481-489).
 //
-// One CTA = 128 queries of one (image, head).  warp0: TMA producer; warp1: single-thread tcgen05.mma issuer;
-// warps 2-5: softmax, one thread per query row (= TMEM lane).  Per 64-key block j:
-//     S_j = Q K_j^T            (tcgen05, fp32 in TMEM, double buffered so S_{j+1} overlaps softmax of S_j)
-//     online softmax in registers, P_j -> ONE fp16 plane -> shared memory (SW128 K-major)
-//     O += P_j V_j             (tcgen05, accumulated IN TMEM across the key blocks; round 2)
-// with LAZY rescaling: exponents are taken against a per-row reference maximum m_ref that only moves when a block's maximum
-// exceeds it by more than 2^8 (then O and l of that row are multiplied by 2^(m_ref_old - m_ref_new): tcgen05.ld -> mul ->
-// tcgen05.st by the warp that owns the rows, before it releases P_j).  Probabilities stay below 2^8 (fp16 holds them at full
-// relative precision), O / l is unchanged mathematically, and the per-block read-back of O (DP tcgen05.ld columns + DP FFMAs
-// per row and block, an o_full / o_empty round trip) of round 1 is gone: after the first blocks the reference rarely moves.
+// One CTA = 128 queries of one (image, head): two consumer warpgroups own 64 query rows each, a producer warpgroup's
+// first thread issues the TMA loads.  Per 64-key block j, in each consumer warpgroup:
+//     S_j = Q K_j^T            (wgmma, both operands in shared memory, fp32 accumulators in registers)
+//     online softmax in registers (a row lives in the 4 lanes of a quad), P_j -> fp16 (bf16x3) / bf16 register fragments
+//     O += P_j V_j             (wgmma with A = P_j from registers, accumulated in registers across the key blocks)
 // Operands are head-padded planes: head h occupies columns [h*HS, h*HS + DP) of q / k and rows of v^T with
 // HS = 64 (d=40, DP=48) or 128 (d=80, DP=80); pad columns are zeros (produced by zero weight rows in the
 // projection GEMM).  bf16x3: S = Q K^T uses hi*hi + hi*lo + lo*hi (the logits are exponentiated); O = P V uses
-// P16 * V_hi + P16 * V_lo with V^T given as fp16 (hi, lo) planes (odise_gemm_desc.out_planes_fp16) and P rounded once to fp16 (p in [0, 1]: 2^-12 relative, random sign, averaged over the keys;
-// measured 9e-5 on the UNet taps by tools/precision_budget.py, bar 1e-3) — one F2FP per pair of probabilities instead of
-// the six-instruction (hi, lo) bf16 split, half the shared-memory stores, two PV MMAs instead of three.
+// P16 * V_hi + P16 * V_lo with V^T given as fp16 (hi, lo) planes (odise_gemm_desc.out_planes_fp16; wgmma multiplies
+// operands of one 16-bit type) and P in [0, 1] rounded once to fp16 (2^-12 relative, random sign, averaged over the keys;
+// bar 1e-3 on the UNet taps).
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "odise_b200.h"
 #include "launch_count.h"
 #include <cuda_fp16.h>
@@ -44,10 +40,10 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
-// DP = width of the P V product one CTA computes (= TMEM / register accumulator width); QK = contraction width of
+// DP = width of the P V product one CTA computes (= register accumulator width); QK = contraction width of
 // Q K^T (head dim padded to 16).  QK > DP: the head's V columns are split over QK / DP CTAs that each recompute S
-// (head dim 160 of the 16x16 / 8x8 UNet levels: QK = 160, DP = 80, two CTAs per (tile, head)) — 160 fp32 accumulators
-// per thread next to the 64 scores would not fit the register file.
+// (head dim 160 of the 16x16 / 8x8 UNet levels: QK = 160, DP = 80, two CTAs per (tile, head)), which keeps Q, one K
+// stage and two V stages of a 160-wide head within shared memory.
 template <int DP, int NMMA, int QK = DP>
 struct AttnCfg {
   static constexpr int NC = (QK + 63) / 64;          // 64-column chunks per head
@@ -55,21 +51,26 @@ struct AttnCfg {
   static constexpr int NP = (NMMA == 3) ? 2 : 1;
   static constexpr int BK = 64;                      // keys per block
   static constexpr int STAGES = (NC >= 3) ? 1 : 2;           // K stages (three chunks: shared memory allows one)
-  // d = 40: one V stage + 256 TMEM columns so that TWO CTAs fit per SM (softmax of one overlaps the MMAs of the other)
-  static constexpr int VSTAGES = (DP <= 64 || NC >= 3) ? 1 : 2;
-  static constexpr int CTAS_PER_SM = (DP <= 64 && NC == 1) ? 2 : 1;   // one fp16 P plane: d = 64 (CLIP) fits twice too
+  static constexpr int VSTAGES = 2;
   static constexpr int Q_BYTES = NC * NP * 128 * 128;       // [chunk][plane][128 rows x 128 B]
   static constexpr int K_BYTES = NC * NP * BK * 128;        // per stage
   static constexpr int V_TILE = DP * 128;                   // one plane: DP rows x 64 tokens
   static constexpr int V_BYTES = NP * V_TILE;               // per stage
-  static constexpr int P_BYTES = 128 * 128;                 // one plane: fp16 (bf16x3 mode) or bf16 (plain bf16 mode)
-  static constexpr int SMEM_BYTES = Q_BYTES + STAGES * K_BYTES + VSTAGES * V_BYTES + P_BYTES + 1024 + 256;
-  static constexpr int OSTRIDE = (DP <= 64) ? 64 : 128;     // TMEM columns per O buffer
-  static constexpr int TMEM_COLS = (DP <= 64) ? 256 : 512;  // S: 2 x 64 @ 0, O: 2 x OSTRIDE @ 128
+  static constexpr int SMEM_BYTES = Q_BYTES + STAGES * K_BYTES + VSTAGES * V_BYTES + 1024 + 256;
+  static constexpr int THREADS = 384;
 };
 
+__device__ __forceinline__ uint32_t pack2(float a, float b, bool f16) {
+  if (f16) {
+    const __half2 h2 = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h2);
+  }
+  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h2);
+}
+
 template <int DP, int NMMA, int QK = DP>
-__global__ void __launch_bounds__(192, AttnCfg<DP, NMMA, QK>::CTAS_PER_SM)
+__global__ void __launch_bounds__(384, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
                const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl,
@@ -80,57 +81,39 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Cfg::Q_BYTES;
   uint8_t* sV = sK + Cfg::STAGES * Cfg::K_BYTES;
-  uint8_t* sP = sV + Cfg::VSTAGES * Cfg::V_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::P_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + Cfg::VSTAGES * Cfg::V_BYTES);
   uint64_t* q_full = bars;            // 1
   uint64_t* k_full = bars + 1;        // [2]
   uint64_t* k_empty = bars + 3;       // [2]
   uint64_t* v_full = bars + 5;        // [2]
   uint64_t* v_empty = bars + 7;       // [2]
-  uint64_t* s_full = bars + 9;        // [2]
-  uint64_t* s_empty = bars + 11;      // [2]
-  uint64_t* o_full = bars + 13;       // [2]
-  uint64_t* o_empty = bars + 15;      // [2]
-  uint64_t* p_full = bars + 17;       // 1
-  uint64_t* p_empty = bars + 18;      // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int VPARTS = QK > DP ? QK / DP : 1;        // CTAs sharing one head (each owns DP columns of V / of the output)
   const int q0 = blockIdx.x * 128, h = blockIdx.y / VPARTS, vpart = blockIdx.y % VPARTS, b = blockIdx.z;
   const int nblk = (p.Tk + Cfg::BK - 1) / Cfg::BK;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQh); tma_prefetch_desc(&tmKh); tma_prefetch_desc(&tmVh);
     mbar_init(q_full, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1);
-      mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], 128);
-      mbar_init(&o_full[s], 1); mbar_init(&o_empty[s], 128);
+      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 8);   // lane 0 of every consumer warp releases a stage
+      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 8);
     }
-    mbar_init(p_full, 128);
-    mbar_init(p_empty, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
       // ---------------------------------------------------------------- TMA producer
       mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
       for (int c = 0; c < Cfg::NC; ++c) {
         tma_load_3d(sQ + (c * Cfg::NP) * 16384, &tmQh, q_full, h * Cfg::HS + c * 64, b * p.Tq + q0, 0);
         if (NMMA == 3) tma_load_3d(sQ + (c * Cfg::NP + 1) * 16384, &tmQl, q_full, h * Cfg::HS + c * 64, b * p.Tq + q0, 0);
       }
-      auto load_k = [&](int j) {
+      for (int j = 0; j < nblk; ++j) {
         const int st = j % Cfg::STAGES;
         mbar_wait(&k_empty[st], ((j / Cfg::STAGES) & 1) ^ 1);
         mbar_arrive_expect_tx(&k_full[st], Cfg::K_BYTES);
@@ -140,10 +123,6 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
           if (NMMA == 3)
             tma_load_3d(kd + (c * Cfg::NP + 1) * 8192, &tmKl, &k_full[st], h * Cfg::HS + c * 64, b * p.TkS + j * 64, 0);
         }
-      };
-      load_k(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) load_k(j + 1);        // K runs one block ahead; V is loaded just in time
         const int sv = j % Cfg::VSTAGES;
         mbar_wait(&v_empty[sv], ((j / Cfg::VSTAGES) & 1) ^ 1);
         mbar_arrive_expect_tx(&v_full[sv], Cfg::V_BYTES);
@@ -153,214 +132,150 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
           tma_load_3d(vd + Cfg::V_TILE, &tmVl, &v_full[sv], b * p.TkS + j * 64, h * Cfg::HS + vpart * DP, 0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ---------------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 64);
-      constexpr uint32_t idesc_o = (NMMA == 3) ? umma_idesc_f16(128, DP) : umma_idesc_bf16(128, DP);
-      constexpr int KS = QK / 16;
-      auto issue_s = [&](int j) {
-        const int st = j & 1;                      // S buffer in TMEM
-        const int sk = j % Cfg::STAGES;            // K stage in shared memory
-        mbar_wait(&k_full[sk], (j / Cfg::STAGES) & 1);
-        mbar_wait(&s_empty[st], ((j >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + st * 64;
-        const uint32_t kq = smem_u32(sQ), kk = smem_u32(sK + sk * Cfg::K_BYTES);
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          const int c = ks >> 2, off = (ks & 3) * 32;
-          const uint64_t qh = umma_desc_sw128(kq + (c * Cfg::NP) * 16384 + off);
-          const uint64_t kh = umma_desc_sw128(kk + (c * Cfg::NP) * 8192 + off);
-          umma_bf16(d_tmem, qh, kh, idesc_s, ks > 0 ? 1u : 0u);
-          if (NMMA == 3) {
-            const uint64_t ql = umma_desc_sw128(kq + (c * Cfg::NP + 1) * 16384 + off);
-            const uint64_t kl = umma_desc_sw128(kk + (c * Cfg::NP + 1) * 8192 + off);
-            umma_bf16(d_tmem, qh, kl, idesc_s, 1u);
-            umma_bf16(d_tmem, ql, kh, idesc_s, 1u);
-          }
-        }
-        umma_commit(&k_empty[sk]);
-        umma_commit(&s_full[st]);
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int j = 0; j < nblk; ++j) {
-        if (j + 1 < nblk) issue_s(j + 1);
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        const int sv = j % Cfg::VSTAGES;
-        mbar_wait(p_full, j & 1);           // P_j written AND (if the reference maximum moved) O rescaled by the softmax warps
-        mbar_wait(&v_full[sv], (j / Cfg::VSTAGES) & 1);
-        tc_fence_after();
-        (void)st; (void)ph;
-        const uint32_t d_tmem = tmem_base + 128;                 // ONE O tile, accumulated over all key blocks
-        const uint32_t pp = smem_u32(sP), vv = smem_u32(sV + sv * Cfg::V_BYTES);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t ph_ = umma_desc_sw128(pp + ks * 32);
-          const uint64_t vh = umma_desc_sw128(vv + ks * 32);
-          umma_bf16(d_tmem, ph_, vh, idesc_o, (j > 0 || ks > 0) ? 1u : 0u);
-          if (NMMA == 3) {
-            const uint64_t vl = umma_desc_sw128(vv + Cfg::V_TILE + ks * 32);
-            umma_bf16(d_tmem, ph_, vl, idesc_o, 1u);
-          }
-        }
-        umma_commit(&v_empty[sv]);
-        umma_commit(p_empty);
-        umma_commit(&o_full[0]);           // one phase per key block (the softmax warps wait on it only when they rescale)
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax / epilogue (thread = query row)
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    float m = -INFINITY, l = 0.f;          // m: the row's REFERENCE maximum (lazy, see the header), l: running sum
-    constexpr float TAU = 8.f;             // the reference moves when a block maximum exceeds it by 2^TAU
-    const int n_words = (p.Tk + 31) / 32;
-    const uint32_t* mask_words = nullptr;
-    if (p.bits && q0 + row < p.Tq && p.row_any[(long long)b * p.Tq + q0 + row] != 0)
-      mask_words = p.bits + ((long long)b * p.Tq + q0 + row) * n_words;
-    const uint32_t t_o = t_lane + 128;
-
-    for (int j = 0; j < nblk; ++j) {
-      const int st = j & 1;
-      mbar_wait(&s_full[st], (j >> 1) & 1);
-      tc_fence_after();
-      float s[64];
-      {
-        uint32_t v[32];
-        tmem_ld32(t_lane + st * 64, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) s[i] = __uint_as_float(v[i]);
-        tmem_ld32(t_lane + st * 64 + 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) s[32 + i] = __uint_as_float(v[i]);
-      }
-      tc_fence_before();
-      mbar_arrive(&s_empty[st]);
-      const int valid = p.Tk - j * 64;  // keys of this block that exist
-      if (valid < 64) {                 // only the last block can be ragged (warp-uniform)
-#pragma unroll
-        for (int i = 0; i < 64; ++i) if (i >= valid) s[i] = -INFINITY;
-      }
-      if (mask_words) {                 // per-row predicted-mask bits (masked cross-attention)
-        const uint32_t w0 = __ldg(mask_words + 2 * j);
-        const uint32_t w1 = (2 * j + 1 < n_words) ? __ldg(mask_words + 2 * j + 1) : 0u;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (!((w0 >> i) & 1u)) s[i] = -INFINITY;
-          if (!((w1 >> i) & 1u)) s[32 + i] = -INFINITY;
-        }
-      }
-      // block maximum of the raw scores (scale > 0): three-input max tree
-      float bm = fmaxf(s[0], s[1]);
-#pragma unroll
-      for (int i = 2; i < 64; i += 2) bm = fmaxf(bm, fmaxf(s[i], s[i + 1]));
-      const float c = p.scale_log2;
-      // lazy reference: move it only when this block would push a probability above 2^TAU (or the row had none yet)
-      const bool move = (bm - m) * c > TAU || (m == -INFINITY && bm != -INFINITY);
-      float alpha = 1.f;
-      if (move) {
-        alpha = (m == -INFINITY) ? 0.f : fast_exp2((m - bm) * c);
-        m = bm;
-      }
-      if (j > 0 && __any_sync(0xffffffffu, move)) {
-        // rescale the rows of this warp in TMEM (lanes whose reference did not move multiply by 1): needs P V of block j - 1
-        mbar_wait(&o_full[0], (j - 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int c0 = 0; c0 < DP; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld16(t_o + c0, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-          tmem_st16(t_o + c0, v);
-        }
-        tmem_st_wait();
-        tc_fence_before();
-      }
-      // guards: a row may have seen no attendable key yet (m = -inf) -> p = 0
-      const float mc = (m == -INFINITY) ? 0.f : -m * c;
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < 64; ++i) {
-        s[i] = fast_exp2(fmaf(s[i], c, mc));
-        sum += s[i];
-      }
-      l = l * alpha + sum;
-      // P_j -> shared memory (SW128 K-major [128 x 64]); wait until PV_{j-1} has finished reading the buffer
-      mbar_wait(p_empty, (j & 1) ^ 1);
-#pragma unroll
-      for (int cch = 0; cch < 8; ++cch) {
-        // bf16x3 mode: p -> fp16 (round to nearest), ONE plane; plain bf16 mode: p -> bf16.  One packed convert per pair.
-        uint32_t hw[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float a0 = s[cch * 8 + 2 * t], a1 = s[cch * 8 + 2 * t + 1];
-          if (NMMA == 3) {
-            const __half2 h2 = __floats2half2_rn(a0, a1);
-            hw[t] = *reinterpret_cast<const uint32_t*>(&h2);
-          } else {
-            const __nv_bfloat162 h2 = __floats2bfloat162_rn(a0, a1);
-            hw[t] = *reinterpret_cast<const uint32_t*>(&h2);
-          }
-        }
-        *reinterpret_cast<uint4*>(sP + sw128_offset(row, cch)) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-      }
-      fence_proxy_async();
-      mbar_arrive(p_full);
-    }
-    // all key blocks accumulated: O of this row out of TMEM once
-    mbar_wait(&o_full[0], (nblk - 1) & 1);
-    tc_fence_after();
-    float acc[DP];
-#pragma unroll
-    for (int c0 = 0; c0 < DP; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld16(t_o + c0, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[c0 + i] = __uint_as_float(v[i]);
-    }
-    tc_fence_before();
-
-    const int q = q0 + row;
-    if (q < p.Tq) {
-      const float inv = 1.f / l;
-      const int dpart = p.d / VPARTS;              // columns of the head this CTA owns
-      const long long o = ((long long)b * p.Tq + q) * p.ldo + (long long)h * p.d + vpart * dpart;
-      if (p.out) {
-#pragma unroll
-        for (int i = 0; i < DP; i += 4)
-          if (i < dpart)
-            *reinterpret_cast<float4*>(p.out + o + i) =
-                make_float4(acc[i] * inv, acc[i + 1] * inv, acc[i + 2] * inv, acc[i + 3] * inv);
-      }
-      if (p.out_hi) {
-#pragma unroll
-        for (int i = 0; i < DP; i += 8) {
-          if (i < dpart) {
-            float ov[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) ov[t] = acc[i + t] * inv;
-            store_planes<8>(p.out_hi + o + i, p.out_lo ? p.out_lo + o + i : nullptr, ov);   // bf16 pair or F16Q8 (tagged lo)
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // ------------------------------------------------------------------ consumer warpgroups (64 query rows each)
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, wi = warp & 3;
+  const int g = lane >> 2, t = lane & 3;
+  // this thread's two rows of the accumulator fragments: g and g + 8 of the warp's 16
+  const int rows[2] = {wg * 64 + wi * 16 + g, wg * 64 + wi * 16 + g + 8};
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const int n_words = (p.Tk + 31) / 32;
+  const uint32_t* mask_words[2] = {nullptr, nullptr};
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q = q0 + rows[hh];
+    if (p.bits && q < p.Tq && p.row_any[(long long)b * p.Tq + q] != 0)
+      mask_words[hh] = p.bits + ((long long)b * p.Tq + q) * n_words;
+  }
+  float o[DP / 2];
+#pragma unroll
+  for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
+  constexpr int KS = QK / 16;
+  const float c = p.scale_log2;
+  const uint32_t kq = smem_u32(sQ) + wg * (64 * 128);
+
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int sk = j % Cfg::STAGES;
+    mbar_wait(&k_full[sk], (j / Cfg::STAGES) & 1);
+    float s[32];
+    const uint32_t kk = smem_u32(sK + sk * Cfg::K_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      const int cc = ks >> 2, off = (ks & 3) * 32;
+      const uint64_t qh = wgmma_desc_sw128(kq + (cc * Cfg::NP) * 16384 + off);
+      const uint64_t kh = wgmma_desc_sw128(kk + (cc * Cfg::NP) * 8192 + off);
+      wgmma_bf16(s, qh, kh, ks > 0 ? 1 : 0);
+      if (NMMA == 3) {
+        wgmma_bf16(s, qh, wgmma_desc_sw128(kk + (cc * Cfg::NP + 1) * 8192 + off), 1);
+        wgmma_bf16(s, wgmma_desc_sw128(kq + (cc * Cfg::NP + 1) * 16384 + off), kh, 1);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    if (lane == 0) mbar_arrive(&k_empty[sk]);
+
+    // s[4 jj + 2 hh + e]: row rows[hh], key 8 jj + 2 t + e of the block
+    const int valid = p.Tk - j * 64;  // keys of this block that exist
+    if (valid < 64) {                 // only the last block can be ragged
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (8 * (i >> 2) + 2 * t + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      if (mask_words[hh]) {           // per-row predicted-mask bits (masked cross-attention)
+        const uint32_t w0 = __ldg(mask_words[hh] + 2 * j);
+        const uint32_t w1 = (2 * j + 1 < n_words) ? __ldg(mask_words[hh] + 2 * j + 1) : 0u;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = 8 * jj + 2 * t + e;
+            const uint32_t w = key < 32 ? w0 : w1;
+            if (!((w >> (key & 31)) & 1u)) s[4 * jj + 2 * hh + e] = -INFINITY;
+          }
+      }
+    }
+    float alpha[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float bm = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) bm = fmaxf(bm, fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
+      bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, 1));
+      bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, 2));
+      const float mn = fmaxf(m[hh], bm);
+      alpha[hh] = (m[hh] == -INFINITY) ? 0.f : fast_exp2((m[hh] - mn) * c);
+      m[hh] = mn;
+      // guards: a row may have seen no attendable key yet (m = -inf) -> p = 0
+      const float mc = (mn == -INFINITY) ? 0.f : -mn * c;
+      float sum = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * jj + 2 * hh + e];
+          v = fast_exp2(fmaf(v, c, mc));
+          sum += v;
+        }
+      l[hh] = l[hh] * alpha[hh] + sum;    // this lane's share of the row sum (the quad is summed at the end)
+    }
+#pragma unroll
+    for (int jj = 0; jj < DP / 8; ++jj) {
+      o[4 * jj] *= alpha[0]; o[4 * jj + 1] *= alpha[0];
+      o[4 * jj + 2] *= alpha[1]; o[4 * jj + 3] *= alpha[1];
+    }
+    // P_j as the A fragments of four k16 slices: the accumulator layout of S is the m64k16 A-fragment layout
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int kk2 = 0; kk2 < 4; ++kk2)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) pa[kk2][r] = pack2(s[8 * kk2 + 2 * r], s[8 * kk2 + 2 * r + 1], NMMA == 3);
+
+    const int sv = j % Cfg::VSTAGES;
+    mbar_wait(&v_full[sv], (j / Cfg::VSTAGES) & 1);
+    const uint32_t vv = smem_u32(sV + sv * Cfg::V_BYTES);
+    reg_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk2 = 0; kk2 < 4; ++kk2) {
+      if (NMMA == 3) {
+        wgmma_rs_f16(o, pa[kk2], wgmma_desc_sw128(vv + kk2 * 32), 1);
+        wgmma_rs_f16(o, pa[kk2], wgmma_desc_sw128(vv + Cfg::V_TILE + kk2 * 32), 1);
+      } else {
+        wgmma_rs_bf16(o, pa[kk2], wgmma_desc_sw128(vv + kk2 * 32), 1);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (lane == 0) mbar_arrive(&v_empty[sv]);
+  }
+
+  const int dpart = p.d / VPARTS;              // columns of the head this CTA owns
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float lt = l[hh];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const int q = q0 + rows[hh];
+    if (q >= p.Tq) continue;
+    const float inv = 1.f / lt;
+    const long long ob = ((long long)b * p.Tq + q) * p.ldo + (long long)h * p.d + vpart * dpart;
+#pragma unroll
+    for (int jj = 0; jj < DP / 8; ++jj) {
+      const int col = 8 * jj + 2 * t;
+      if (col >= dpart) continue;
+      float ov[2] = {o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv};
+      if (p.out) *reinterpret_cast<float2*>(p.out + ob + col) = make_float2(ov[0], ov[1]);
+      if (p.out_hi) store_planes<2>(p.out_hi + ob + col, p.out_lo ? p.out_lo + ob + col : nullptr, ov);   // bf16 pair or F16Q8
+    }
   }
 }
 
@@ -403,7 +318,7 @@ static int attn_launch(const CUtensorMap* m, const AttnParams& p, cudaStream_t s
     attr_set = true;
   }
   dim3 grid((p.Tq + 127) / 128, p.heads * (QK > DP ? QK / DP : 1), p.B);
-  attn_tc_kernel<DP, NMMA, QK><<<grid, 192, Cfg::SMEM_BYTES, stream>>>(m[0], m[1], m[2], m[3], m[4], m[5], p);
+  attn_tc_kernel<DP, NMMA, QK><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(m[0], m[1], m[2], m[3], m[4], m[5], p);
   return (int)cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// HBM-bound elementwise / normalisation passes of the ODISE hot path (sm_100a).  Activations are NHWC /
+// HBM-bound elementwise / normalisation passes of the ODISE hot path (sm_90a).  Activations are NHWC /
 // token-major fp32; every pass that feeds a GEMM also writes the (hi, lo) bf16 operand planes, so the
 // fp32 -> bf16x2 split is never a pass of its own.  Reference ops replaced (all individual ATen kernels in
 // the reference, SURVEY.md §2.4 "Fused ops: none"): nn.GroupNorm + SiLU (ldm ResBlock / Normalize),
@@ -17,7 +17,8 @@ namespace ob {
 static std::atomic<long long> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
-static inline int grid_for(long long work, int threads, int max_blocks = 148 * 16) {
+static inline int grid_for(long long work, int threads, int max_blocks = 0) {
+  if (max_blocks <= 0) max_blocks = num_sms() * 16;
   long long b = (work + threads - 1) / threads;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -153,7 +154,8 @@ gn_stats_kernel(const float* __restrict__ x, long long ldx, float* __restrict__ 
 
 // grid (pixel chunks, B); thread = fixed channel quad (+ pixel lane): the per-channel constants
 // (mean, rstd, gamma, beta of the quad) are loaded once, the inner loop is load / 2 FMA-class ops / act / store.
-__global__ void gn_apply_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ mean,
+// Up to 1024 threads (C = 4096): the bound keeps the register count launchable.
+__global__ void __launch_bounds__(1024) gn_apply_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ mean,
                                 const float* __restrict__ rstd, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, int act, float* __restrict__ y, long long ldy,
                                 __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, long long ldo,
@@ -294,7 +296,7 @@ static int launch_gn_apply(const float* x, long long ldx, const float* mean, con
     const int C8 = C / 8;
     const int PL = 256 / C8;
     const int threads = C8 * PL;
-    int chunks = (4 * 148 + B - 1) / B;          // one resident wave: 4 blocks per SM
+    int chunks = (4 * num_sms() + B - 1) / B;          // one resident wave: 4 blocks per SM
     if (chunks > (HW + 2 * PL - 1) / (2 * PL)) chunks = (HW + 2 * PL - 1) / (2 * PL);
     if (chunks < 1) chunks = 1;
     const int ppb = (HW + chunks - 1) / chunks;
@@ -308,7 +310,7 @@ static int launch_gn_apply(const float* x, long long ldx, const float* mean, con
   int PL = 256 / C4;
   if (PL < 1) PL = 1;
   const int threads = C4 * PL;
-  int chunks = (6 * 148 + B - 1) / B;            // ~6 blocks per SM
+  int chunks = (6 * num_sms() + B - 1) / B;            // ~6 blocks per SM
   if (chunks > (HW + PL - 1) / PL) chunks = (HW + PL - 1) / PL;
   if (chunks < 1) chunks = 1;
   const int ppb = (HW + chunks - 1) / chunks;
@@ -1274,7 +1276,7 @@ extern "C" int odise_image_crops_u8_f32(const uint8_t* img, float* out, const in
 // workspace-based, coalesced statistics (see gn_partial_kernel).  ws: >= odise_groupnorm_ws_floats(B, HW, C, G) floats.
 extern "C" long long odise_groupnorm_ws_floats(int B, int HW, int C, int G) {
   (void)C;
-  int nchunk = (4 * 148 + B - 1) / B;
+  int nchunk = (4 * num_sms() + B - 1) / B;
   if (nchunk > HW) nchunk = HW;
   if (nchunk < 1) nchunk = 1;
   return (long long)B * nchunk * G * 2;
@@ -1284,7 +1286,7 @@ extern "C" int odise_groupnorm_stats_ws_f32(const float* x, long long ldx, long 
                                             float* rstd, int B, int HW, int C, int G, float eps, void* stream) {
   if (!x || !ws || !mean || !rstd || B <= 0 || HW <= 0 || C <= 0 || G <= 0 || C % G) return ODISE_ERR_ARG;
   if (C % 4 || ldx % 4 || x_bs % 4 || C / 4 > 1024) return ODISE_ERR_ALIGN;
-  int nchunk = (4 * 148 + B - 1) / B;
+  int nchunk = (4 * num_sms() + B - 1) / B;
   if (nchunk > HW) nchunk = HW;
   if (nchunk < 1) nchunk = 1;
   const int ppc = (HW + nchunk - 1) / nchunk;

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a: the tensor-core workhorse behind every dense contraction on the ODISE
+// wgmma / TMA GEMM for sm_90a: the tensor-core workhorse behind every dense contraction on the ODISE
 // inference hot path (SURVEY.md §8a rows a7.1 ResBlock convs, a7.2 transformer linears, a3 projections,
 // b2-b4 pixel-decoder linears, b8-b10 decoder linears / mask einsum / pooling, b12 CLIP match).
 //
@@ -9,15 +9,19 @@
 //   K loop walks (kh, kw, c-chunk) and lets TMA's out-of-bounds zero fill implement the padding.
 //   (reference op: F.conv2d inside ldm ResBlock, call sites odise/modeling/meta_arch/ldm.py:481-489)
 // * precision: NMMA=1 plain bf16, NMMA=3 "bf16x3": operands carry a (hi, lo) bf16 pair per fp32 value and the
-//   kernel issues hi*hi + hi*lo + lo*hi into the same fp32 TMEM accumulator (~16 mantissa bits, the mode that
+//   kernel issues hi*hi + hi*lo + lo*hi into the same fp32 accumulator (~16 mantissa bits, the mode that
 //   meets the 1e-3 fp32 parity bar of BASELINE.json; see DESIGN.md).  NMMA=2 "f16q8" (ptx.cuh, ODISE_PLANES_F16Q8):
-//   hi = fp16 plane, second plane = e5m2 bytes [x * 2^-6 | (x - hi) * 2^6] per 64-wide k-block; per k-block 4 kind::f16
-//   MMAs (hi*hi) + 4 kind::f8f6f4 MMAs (the two cross terms, K = 32 each, twice the MAC rate) into the same accumulator:
-//   8 instruction slots instead of 12, same shared-memory bytes, ~14 mantissa bits.
-// * persistent, warp-specialised: warp0 = TMA producer, warp1 = single-thread tcgen05.mma issuer, warps 2-5 =
-//   epilogue (tcgen05.ld -> bias / per-image row bias / residual / activation -> fp32 and/or (hi,lo) bf16 stores).
-//   Two TMEM accumulator stages let the epilogue of tile i overlap the main loop of tile i+1.
+//   hi = fp16 plane, second plane = e5m2 bytes [x * 2^-6 | (x - hi) * 2^6] per 64-wide k-block; per k-block 4 fp16
+//   MMAs (hi*hi) + 4 e5m2 MMAs (the two cross terms, K = 32 each, twice the MAC rate) into the same accumulator:
+//   8 instruction slots instead of 12, same shared-memory bytes, ~14 mantissa bits.  The e5m2 MMAs accumulate into a
+//   register array of their own, added to the fp16 one at the end of the tile: an 8-bit wgmma adds into its accumulator
+//   at reduced precision, which would truncate the hi*hi sum.  Two accumulators fit the register file up to BN = 128, so
+//   F16Q8 runs 64- and 128-wide tiles.
+// * persistent, warp-specialised: one TMA producer warp fills a ring of shared-memory stages; two consumer warpgroups
+//   run wgmma on 64 rows each of a 128 x BN tile and then its epilogue (bias / per-image row bias / residual /
+//   activation / GEGLU / GroupNorm records -> fp32 and/or (hi, lo) plane stores).
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "odise_b200.h"
 #include "launch_count.h"
 #include <cudaTypedefs.h>
@@ -37,11 +41,6 @@ struct GemmParams {
   int nseg;                        // > 1: the 128 pixels of a tile are fetched as nseg row segments of bw pixels
   int cstride, cpad;               // conv stride (1 | 2) and low-side zero padding (0 | 1)
   int tiles_m, tiles_n, splits, kblocks;
-  // cl = 2: CTA pairs (cluster of 2 along M) work on the two M tiles {2i, 2i+1} of one n-tile in lock step; each CTA fetches
-  // half of the shared B tile and TMA-multicasts it to both -> one third fewer operand bytes through L2 / the crossbar per
-  // FLOP (ncu r2g: the K = 4608 GEMM delivers 7.25 GB at ~6 800 B/clk chip-wide = the L2 -> SM delivery ceiling, tensor pipe
-  // 65 % (bf16x3) / 48 % (F16Q8) active).  tiles_mp = M tiles per CTA of the cluster (= ceil(tiles_m / cl)).
-  int cl, tiles_mp;
   float alpha;
   const float* bias;
   const float* bias_m;  // per-row (m) bias, for swapped-operand (transposed-output) projections
@@ -68,9 +67,6 @@ struct GemmParams {
   // in fixed order (Chan's formula, double) -> no atomics, bit-reproducible, no second pass over the activation.
   float* gnp;
   long long gnp_seg, gnp_plane;
-  // 1: interior tiles leave through TMA stores (registers -> swizzled shared staging -> cp.async.bulk.tensor store issued by
-  // one lane; no per-thread global addressing, full-line writes); 2: the same for the (hi, lo) planes instead of fp32
-  int tma_out;
 };
 
 // 4 columns x the 4 rows a lane owns -> per-column (shift, S1, S2) of the warp's 32 rows; lanes 0..3 (rsub == 0) hold
@@ -222,61 +218,46 @@ __device__ __forceinline__ void epilogue_quad(const GemmParams& p, int z, int m,
   }
 }
 
-// SM2 = 1: the CTA pair runs cta_group::2 MMAs (M = 256 over the two CTAs' TMEM); each CTA keeps only ITS half of the B tile
-// (BN / 2 rows) in shared memory -> smaller stages (3 instead of 2 at BN = 256) and one third fewer operand bytes delivered
-// per FLOP.
-template <int BN, int NMMA, int SM2 = 0>
+// Two consumer warpgroups (rows [0, 64) and [64, 128) of the tile, fp32 accumulators in registers) and a producer
+// warpgroup whose first thread issues the TMA loads (the rest of it only hands its registers to the consumers).  The epilogue scatters the accumulator fragments, 32 columns at a time, into per-warp [32 rows x 16 fp32] staging
+// blocks (XOR swizzled) so that every warp then owns 32 whole rows x 16 columns: coalesced global accesses (8 rows x 64
+// contiguous bytes per warp-level access) and the 32-row GroupNorm segments.
+template <int BN, int NMMA>
 struct GemmCfg {
   static constexpr int BM = 128, BK = 64;
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (SM2 ? BN / 2 : BN) * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int PLANES = (NMMA == 1) ? 1 : 2;
   static constexpr int STAGE_BYTES = PLANES * (A_BYTES + B_BYTES);
-  // epilogue warps: one warp per scheduler is latency bound (ncu: IPC 0.17/warp), so two warps share each TMEM lane
-  // quadrant and alternate 16-column chunks; BN=160/bf16x3 has no shared memory left for the second set
-  static constexpr int NEPI = (BN == 160 && NMMA != 1) ? 4 : 8;
-  static constexpr int THREADS = 64 + 32 * NEPI;
-  // per warp [32 rows x 16 fp32] staging (XOR swizzled); doubled where shared memory allows so that the TMA store of
-  // chunk i can still be reading its buffer while chunk i + 1 is written
-  static constexpr int EPI_BUFS = (BN == 160 && NMMA != 1) ? 1 : 2;
-  static constexpr int EPI_PER_WARP = EPI_BUFS * 32 * 16 * 4;
-  static constexpr int EPI_BYTES = NEPI * EPI_PER_WARP;
-  static constexpr int STAGES_RAW = (232448 - EPI_BYTES - 256) / STAGE_BYTES;
+  static constexpr int THREADS = 384;
+  static constexpr int EPI_BYTES = 8 * 32 * 16 * 4;
+  // 227 KB per block on H100, minus the epilogue staging, barriers and the slack for aligning the base to 1024 B
+  static constexpr int STAGES_RAW = (232448 - EPI_BYTES - 256 - 1024) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int ACC_STRIDE = (BN <= 64) ? 64 : (BN <= 128 ? 128 : 256);  // TMEM columns per accumulator
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 /*barriers: 3 * STAGES + 4 of 8 B + TMEM slot*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 256 + 1024;
+  static_assert(STAGES >= 2, "GEMM tile does not fit shared memory");
 };
 
 // EPI selects the compiled epilogue of the interior fast path (the runtime flags it excludes are guaranteed off by the
 // host dispatch): 0 = lean (alpha, bias, activation -> fp32 and/or planes), 1 = + row bias / bias_m / residual,
-// 2 = fused GEGLU.  ncu on the K = 320 FF1 GEMM showed ~190 of the 354 instructions of a chunk iteration were runtime
-// flag tests, predicated-off adds and parameter re-loads; the lean variant drops them.
-template <int BN, int NMMA, int EPI, int SM2>
-__global__ void __launch_bounds__(GemmCfg<BN, NMMA, SM2>::THREADS, 1)
+// 2 = fused GEGLU.
+template <int BN, int NMMA, int EPI>
+__global__ void __launch_bounds__(GemmCfg<BN, NMMA>::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-               const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1,
-               const GemmParams p) {
-  using Cfg = GemmCfg<BN, NMMA, SM2>;
-  extern __shared__ __align__(1024) uint8_t smem[];   // SWIZZLE_128B tiles need 1024-byte alignment
+               const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, const GemmParams p) {
+  using Cfg = GemmCfg<BN, NMMA>;
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B tiles need 1024-byte alignment
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* epi_smem = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::EPI_BYTES);
   uint64_t* full = bars;                       // [STAGES]
   uint64_t* empty = bars + Cfg::STAGES;        // [STAGES]
-  uint64_t* tfull = bars + 2 * Cfg::STAGES;    // [2]
-  uint64_t* tempty = bars + 2 * Cfg::STAGES + 2;  // [2]
-  uint64_t* full2 = bars + 2 * Cfg::STAGES + 4;   // [STAGES]  SM2, leader CTA: "the peer's half of stage s has landed"
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * Cfg::STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
-    if (smem_u32(smem) & 1023u) {
-      printf("odise_b200: dynamic shared memory base not 1024-byte aligned\n");
-      __trap();
-    }
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmAh);
     tma_prefetch_desc(&tmBh);
     if (NMMA != 1) {
@@ -285,45 +266,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
     }
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      // multicast pairs: one tcgen05.commit arrival per CTA that reads the stage; SM2: the leader's (multicast) commit only
-      mbar_init(&empty[s], SM2 ? 1 : p.cl);
-      mbar_init(&full2[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], (SM2 ? 2 : 1) * 32 * Cfg::NEPI);   // SM2: the epilogue warps of BOTH CTAs release the pair's accumulator
+      mbar_init(&empty[s], 8);   // lane 0 of every consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (SM2) { tmem_alloc2(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish2(); }
-    else { tmem_alloc(tmem_slot, Cfg::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (p.cl > 1) cluster_sync();        // the peer's barriers are initialised before any multicast / remote arrival
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int crank = p.cl > 1 ? (int)cluster_ctarank() : 0;
 
-  // (pair mode: "tile" counts PAIRS of M tiles; both CTAs of a cluster walk the same sequence)
-  const int tiles_per_z = p.tiles_mp * p.tiles_n * p.splits;
+  const int tiles_per_z = p.tiles_m * p.tiles_n * p.splits;
   const int total_tiles = tiles_per_z * p.batch;
-  const int first_tile = (int)blockIdx.x / p.cl, tile_step = (int)gridDim.x / p.cl;
   const int kb_per_split = (p.kblocks + p.splits - 1) / p.splits;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
       // ------------------------------------------------------------ TMA producer
       int stage = 0;
       uint32_t phase = 0;
       const int cpk = p.conv ? (p.C / 64) : 1;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int z = tile / tiles_per_z;
         int r = tile - z * tiles_per_z;
-        const int sp = r / (p.tiles_mp * p.tiles_n);
-        r -= sp * (p.tiles_mp * p.tiles_n);
-        const int mt = (r / p.tiles_n) * p.cl + crank, nt = r % p.tiles_n;
+        const int sp = r / (p.tiles_m * p.tiles_n);
+        r -= sp * (p.tiles_m * p.tiles_n);
+        const int mt = r / p.tiles_n, nt = r % p.tiles_n;
         const int m0 = mt * 128, n0 = nt * BN;
         const int kb0 = sp * kb_per_split;
         const int kb1 = min(p.kblocks, kb0 + kb_per_split);
@@ -367,442 +332,236 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__
           }
           const int zb = p.b_batched ? z : 0;
           uint8_t* sb = st + Cfg::PLANES * Cfg::A_BYTES;
-          if (SM2) {
-            // 2-SM MMA: this CTA keeps rows [crank * BN/2, +BN/2) of the B tile only (tensor-map box = BN/2 rows)
-            tma_load_3d(sb, &tmBh, &full[stage], kb * 64, n0 + crank * (BN / 2), zb);
-            if (NMMA != 1) tma_load_3d(sb + Cfg::B_BYTES, &tmBl, &full[stage], kb * 64, n0 + crank * (BN / 2), zb);
-          } else if (p.cl == 1) {
-            tma_load_3d(sb, &tmBh, &full[stage], kb * 64, n0, zb);
-            if (NMMA != 1) tma_load_3d(sb + Cfg::B_BYTES, &tmBl, &full[stage], kb * 64, n0, zb);
-          } else {
-            // this CTA's half of the B tile (rows [crank * BN/2, +BN/2), box = BN/2 rows), delivered to both CTAs of the pair
-            constexpr int HB = BN / 2;
-            uint8_t* sh = sb + crank * HB * 128;
-            tma_load_3d_mc(sh, &tmBh, &full[stage], kb * 64, n0 + crank * HB, zb, (uint16_t)3);
-            if (NMMA != 1) tma_load_3d_mc(sh + Cfg::B_BYTES, &tmBl, &full[stage], kb * 64, n0 + crank * HB, zb, (uint16_t)3);
-          }
+          tma_load_3d(sb, &tmBh, &full[stage], kb * 64, n0, zb);
+          if (NMMA != 1) tma_load_3d(sb + Cfg::B_BYTES, &tmBl, &full[stage], kb * 64, n0, zb);
           if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && SM2 && crank == 1) {
-      // ------------------------------------------------------------ odd CTA of a 2-SM pair: no MMAs to issue; it tells the
-      // leader when ITS half of each stage has landed (the leader's MMAs read both CTAs' shared memory)
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        int r = tile % tiles_per_z;
-        const int sp = r / (p.tiles_mp * p.tiles_n);
-        const int kb0 = sp * kb_per_split;
-        const int kb1 = min(p.kblocks, kb0 + kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          mbar_arrive_remote(mapa_shared(&full2[stage], 0));
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    } else if (lane == 0) {
-      // ------------------------------------------------------------ MMA issuer (one thread; SM2: of the even CTA)
-      constexpr uint32_t MM = SM2 ? 256 : 128;
-      constexpr uint32_t idesc = NMMA == 2 ? umma_idesc_f16(MM, BN) : umma_idesc_bf16(MM, BN);
-      constexpr uint32_t idesc_q = umma_idesc_e5m2(MM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t accphase = 0;
-      for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-        int r = tile % tiles_per_z;
-        const int sp = r / (p.tiles_mp * p.tiles_n);
-        const int kb0 = sp * kb_per_split;
-        const int kb1 = min(p.kblocks, kb0 + kb_per_split);
-        if (SM2) mbar_wait_cluster(&tempty[acc], accphase ^ 1);
-        else mbar_wait(&tempty[acc], accphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::ACC_STRIDE;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          if (SM2) mbar_wait_cluster(&full2[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::PLANES * Cfg::A_BYTES;
+    return;
+  }
+
+  // ---------------------------------------------------------------- consumer warpgroups: MMAs, then the epilogue
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, wi = warp & 3;
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  float acc2[BN / 2];                          // F16Q8: the e5m2 cross terms
+  float* stg_wg = epi_smem + wg * (4 * 512);   // the warpgroup's four [32 x 16] staging blocks
+  float* stg = stg_wg + wi * 512;              // the block this warp reads back: rows (wi & 1) * 32, columns (wi >> 1) * 16
+  const int cq = lane & 3, rsub = lane >> 2;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int z = tile / tiles_per_z;
+    int r = tile - z * tiles_per_z;
+    const int sp = r / (p.tiles_m * p.tiles_n);
+    r -= sp * (p.tiles_m * p.tiles_n);
+    const int mt = r / p.tiles_n, nt = r % p.tiles_n;
+    const int n0 = nt * BN;
+    const int kb0 = sp * kb_per_split;
+    const int kb1 = min(p.kblocks, kb0 + kb_per_split);
+
+    // ---- main loop: one k-block of MMAs in flight while the next stage is waited for
+    if (kb0 >= kb1) {   // a split with no k-blocks contributes zeros
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t a_hi = umma_desc_sw128(sa + k * 32);
-            const uint64_t b_hi = umma_desc_sw128(sb + k * 32);
-            const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
-            if (SM2) umma2_f16(d_tmem, a_hi, b_hi, idesc, accum); else umma_bf16(d_tmem, a_hi, b_hi, idesc, accum);
-            if (NMMA == 3) {
-              const uint64_t a_lo = umma_desc_sw128(sa + Cfg::A_BYTES + k * 32);
-              const uint64_t b_lo = umma_desc_sw128(sb + Cfg::B_BYTES + k * 32);
-              if (SM2) { umma2_f16(d_tmem, a_hi, b_lo, idesc, 1u); umma2_f16(d_tmem, a_lo, b_hi, idesc, 1u); }
-              else { umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u); umma_bf16(d_tmem, a_lo, b_hi, idesc, 1u); }
-            }
-          }
-          if (NMMA == 2) {
-            // cross terms on the 8-bit pipe: the second plane of a stage is [q_hi: 64 B | q_lo: 64 B] per row, i.e. 32-byte
-            // chunks 0,1 = q_hi(k 0..31 | 32..63), chunks 2,3 = q_lo;  A.q_hi * B.q_lo + A.q_lo * B.q_hi
-            const uint32_t a2 = sa + Cfg::A_BYTES, b2 = sb + Cfg::B_BYTES;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      if constexpr (NMMA == 2) {
 #pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const uint64_t ah = umma_desc_sw128(a2 + k * 32), bl = umma_desc_sw128(b2 + 64 + k * 32);
-              const uint64_t al = umma_desc_sw128(a2 + 64 + k * 32), bh = umma_desc_sw128(b2 + k * 32);
-              if (SM2) { umma2_f8(d_tmem, ah, bl, idesc_q, 1u); umma2_f8(d_tmem, al, bh, idesc_q, 1u); }
-              else { umma_f8(d_tmem, ah, bl, idesc_q, 1u); umma_f8(d_tmem, al, bh, idesc_q, 1u); }
-            }
-          }
-          // smem slot reusable once these MMAs retire (pair mode: once the MMAs of BOTH CTAs have read their copy)
-          if (SM2) umma2_commit_mc(&empty[stage], (uint16_t)3);
-          else if (p.cl == 1) umma_commit(&empty[stage]);
-          else umma_commit_mc(&empty[stage], (uint16_t)3);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-        // accumulator complete -> epilogue (SM2: the epilogue warps of both CTAs, each on its own 128 rows)
-        if (SM2) umma2_commit_mc(&tfull[acc], (uint16_t)3);
-        else umma_commit(&tfull[acc]);
-        if (++acc == 2) { acc = 0; accphase ^= 1; }
+        for (int i = 0; i < BN / 2; ++i) acc2[i] = 0.f;
       }
     }
-  } else {
-    // -------------------------------------------------------------- epilogue warps (4 x 32 rows)
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may touch
-    int acc = 0;
-    uint32_t accphase = 0;
-    uint32_t tma_cnt = 0;       // chunks this warp has sent through TMA stores (staging buffer parity / group accounting)
-    if (p.tma_out && lane == 0) {
-      tma_prefetch_desc(&tmO0);
-      if (p.tma_out == 2 && p.Dl) tma_prefetch_desc(&tmO1);
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * (64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::PLANES * Cfg::A_BYTES);
+      reg_fence(acc);
+      if constexpr (NMMA == 2) reg_fence(acc2);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t a_hi = wgmma_desc_sw128(sa + k * 32);
+        const uint64_t b_hi = wgmma_desc_sw128(sb + k * 32);
+        const int accum = (kb > kb0 || k > 0) ? 1 : 0;
+        if constexpr (NMMA == 2) wgmma_f16(acc, a_hi, b_hi, accum);
+        else wgmma_bf16(acc, a_hi, b_hi, accum);
+        if constexpr (NMMA == 3) {
+          wgmma_bf16(acc, a_hi, wgmma_desc_sw128(sb + Cfg::B_BYTES + k * 32), 1);
+          wgmma_bf16(acc, wgmma_desc_sw128(sa + Cfg::A_BYTES + k * 32), b_hi, 1);
+        }
+      }
+      if constexpr (NMMA == 2) {
+        // cross terms on the 8-bit MMAs: the second plane of a stage is [q_hi: 64 B | q_lo: 64 B] per row, i.e. 32-byte
+        // chunks 0,1 = q_hi(k 0..31 | 32..63), chunks 2,3 = q_lo;  A.q_hi * B.q_lo + A.q_lo * B.q_hi
+        const uint32_t a2 = sa + Cfg::A_BYTES, b2 = sb + Cfg::B_BYTES;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          wgmma_e5m2(acc2, wgmma_desc_sw128(a2 + k * 32), wgmma_desc_sw128(b2 + 64 + k * 32), (kb > kb0 || k > 0) ? 1 : 0);
+          wgmma_e5m2(acc2, wgmma_desc_sw128(a2 + 64 + k * 32), wgmma_desc_sw128(b2 + k * 32), 1);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                        // the previous k-block's MMAs are done: its stage may be refilled
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
     }
-    for (int tile = first_tile; tile < total_tiles; tile += tile_step) {
-      const int z = tile / tiles_per_z;
-      int r = tile - z * tiles_per_z;
-      const int sp = r / (p.tiles_mp * p.tiles_n);
-      r -= sp * (p.tiles_mp * p.tiles_n);
-      const int mt = (r / p.tiles_n) * p.cl + crank, nt = r % p.tiles_n;
-      const int n0 = nt * BN;
-      mbar_wait(&tfull[acc], accphase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + acc * Cfg::ACC_STRIDE + ((uint32_t)(quad * 32) << 16);
-      const int kb0 = sp * kb_per_split;
-      const bool has_k = kb0 < p.kblocks;  // a split with no k-blocks contributes zeros
-      // TMEM -> registers (thread = row) -> XOR-swizzled shared staging -> coalesced epilogue: each warp-level
-      // global access covers 8 rows x 64 contiguous bytes (full 32-byte sectors) instead of 32 rows x 16 bytes.
-      float* stg = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(epi_smem) + (warp - 2) * Cfg::EPI_PER_WARP);
-      const int m_base = mt * 128 + quad * 32;
-      const int c_first = (Cfg::NEPI == 8 && warp >= 6) ? 16 : 0;
-      const int c_step = (Cfg::NEPI == 8) ? 32 : 16;
-      const int cq = lane & 3, rsub = lane >> 2;
-      const bool interior = p.vec_ok && p.splits == 1 && (mt * 128 + 128 <= p.M) && (n0 + BN <= p.N);
-      if (interior && EPI != 2 && p.tma_out) {
-        // ---- TMA-store epilogue: thread = output row (its TMEM lane), 16 consecutive columns per chunk
-        constexpr bool EXTRA = EPI == 1;
-        const long long m = m_base + lane;
-        const float* rbp = (EXTRA && p.rowbias)
-                               ? p.rowbias + (((long long)z * p.M + m) / p.rows_per_group) * p.rowbias_ld + n0 : nullptr;
-        const float bm = (EXTRA && p.bias_m) ? __ldg(p.bias_m + m) : 0.f;
-        const float* resp = (EXTRA && p.res) ? p.res + (long long)z * p.res_bs + m * p.ldres + n0 : nullptr;
-        const int act = p.act;
-        const float alpha = p.alpha;
-        const bool planes = p.tma_out == 2, to_lo = p.Dl != nullptr, h16 = p.h16 != 0, q8 = lo_is_q8(p.Dl);
-        uint8_t* wbase = reinterpret_cast<uint8_t*>(stg);
-        // residual: each thread reads 64 contiguous bytes of ITS row per chunk, a full memory latency per chunk in this
-        // un-pipelined loop (K <= 640 GEMMs with a residual are epilogue bound) -> the next chunk's bytes are requested into L1
-        // one chunk ahead (a prefetch costs no registers; a register double buffer spilled, ptxas r2r)
-        if (EXTRA && resp) asm volatile("prefetch.global.L1 [%0];" ::"l"(resp + c_first));
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    if constexpr (NMMA == 2) {
+      reg_fence(acc2);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] += acc2[i];
+    }
+
+    // ---- epilogue
+    const int m_base = mt * 128 + wg * 64 + (wi & 1) * 32;
+    const bool interior = p.vec_ok && p.splits == 1 && (mt * 128 + 128 <= p.M) && (n0 + BN <= p.N);
+    constexpr bool EXTRA = EPI == 1, GEGLU = EPI == 2;
+    const bool has_bias = p.bias != nullptr, has_res = EXTRA && p.res != nullptr;
+    const bool to_f32 = p.D != nullptr, to_hi = p.Dh != nullptr, to_lo = p.Dl != nullptr;
+    const int act = p.act;
+    const float alpha = p.alpha;
+    const bool has_gn = !GEGLU && p.gnp != nullptr;
+    const long long gn_seg = ((long long)z * p.M + m_base) >> 5;
 #pragma unroll 1
-        for (int c0 = c_first; c0 < BN; c0 += c_step) {
-          uint32_t v[16];
-          tmem_ld16(t_row + c0, v);
-          if (EXTRA && resp && c0 + c_step < BN) asm volatile("prefetch.global.L1 [%0];" ::"l"(resp + c0 + c_step));
-          float e[16];
-          float4 b4[4];
+    for (int ch = 0; ch < BN / 32; ++ch) {
+      named_bar_sync(1 + wg, 128);          // the previous chunk's staging has been read
+      // fragment of n8 block j: rows wi * 16 + rsub (+ 8), columns 8 j + 2 cq (+ 1)
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-            b4[j] = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-          tmem_ld_wait();
+      for (int j = 0; j < BN / 8; ++j) {
+        if ((j >> 2) != ch) continue;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            e[4 * j + 0] = fmaf(__uint_as_float(v[4 * j + 0]), alpha, b4[j].x + bm);
-            e[4 * j + 1] = fmaf(__uint_as_float(v[4 * j + 1]), alpha, b4[j].y + bm);
-            e[4 * j + 2] = fmaf(__uint_as_float(v[4 * j + 2]), alpha, b4[j].z + bm);
-            e[4 * j + 3] = fmaf(__uint_as_float(v[4 * j + 3]), alpha, b4[j].w + bm);
-          }
-          if (EXTRA && rbp) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 rb = __ldg(reinterpret_cast<const float4*>(rbp + c0) + j);
-              e[4 * j] += rb.x; e[4 * j + 1] += rb.y; e[4 * j + 2] += rb.z; e[4 * j + 3] += rb.w;
-            }
-          }
-          if (act != ODISE_ACT_NONE) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) e[j] = apply_act(e[j], act);
-          }
-          if (EXTRA && resp) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 r4 = *(reinterpret_cast<const float4*>(resp + c0) + j);
-              e[4 * j] += r4.x; e[4 * j + 1] += r4.y; e[4 * j + 2] += r4.z; e[4 * j + 3] += r4.w;
-            }
-          }
-          // staging buffer: wait until the store that last used it has read it
-          const uint32_t sb = (Cfg::EPI_BUFS == 2) ? (tma_cnt & 1u) : 0u;
-          if (tma_cnt >= (uint32_t)Cfg::EPI_BUFS) {
-            if (lane == 0) tma_store_wait_read<Cfg::EPI_BUFS - 1>();
-            __syncwarp();
-          }
-          uint8_t* buf = wbase + sb * 2048;
-          if (!planes) {
-            // [32 rows][16 fp32] = 64-byte rows in the CU_TENSOR_MAP_SWIZZLE_64B pattern: 16-byte chunk ^= (row >> 1) & 3
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<float4*>(buf + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)) =
-                  make_float4(e[4 * j], e[4 * j + 1], e[4 * j + 2], e[4 * j + 3]);
-          } else {
-            // hi plane at +0, lo plane at +1024: [32 rows][16 x 16 bit] = 32-byte rows, SWIZZLE_32B: chunk ^= (row >> 2) & 1
-            uint32_t hw[8], lw[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float a0 = e[2 * j], a1 = e[2 * j + 1];
-              if (q8) {
-                // F16Q8: fp16 hi + e5m2 bytes; lw[0..3] = q_hi of the 16 columns, lw[4..7] = q_lo (two byte pairs per word)
-                const __half2 h2 = __floats2half2_rn(clamp_f16(a0), clamp_f16(a1));
-                hw[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                const float2 f = __half22float2(h2);
-                const uint32_t qh = e5m2x2(a0 * kQ8Down, a1 * kQ8Down), ql = e5m2x2((a0 - f.x) * kQ8Up, (a1 - f.y) * kQ8Up);
-                if (j & 1) { lw[j >> 1] |= qh << 16; lw[4 + (j >> 1)] |= ql << 16; }
-                else { lw[j >> 1] = qh; lw[4 + (j >> 1)] = ql; }
-              } else if (h16) {
-                const __half2 h2 = __floats2half2_rn(a0, a1);
-                hw[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                const float2 f = __half22float2(h2);
-                const __half2 l2 = __floats2half2_rn(a0 - f.x, a1 - f.y);
-                lw[j] = *reinterpret_cast<const uint32_t*>(&l2);
-              } else {
-                const __nv_bfloat162 h2 = __floats2bfloat162_rn(a0, a1);
-                hw[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                const float2 f = __bfloat1622float2(h2);
-                const __nv_bfloat162 l2 = __floats2bfloat162_rn(a0 - f.x, a1 - f.y);
-                lw[j] = *reinterpret_cast<const uint32_t*>(&l2);
-              }
-            }
-            const uint32_t sw = (lane >> 2) & 1u;
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              *reinterpret_cast<uint4*>(buf + lane * 32 + ((c ^ sw) << 4)) =
-                  make_uint4(hw[4 * c], hw[4 * c + 1], hw[4 * c + 2], hw[4 * c + 3]);
-              if (q8)         // [32 rows][16 B] q_hi at +1024, q_lo at +1536, no swizzle (16-byte boxes)
-                *reinterpret_cast<uint4*>(buf + 1024 + c * 512 + lane * 16) =
-                    make_uint4(lw[4 * c], lw[4 * c + 1], lw[4 * c + 2], lw[4 * c + 3]);
-              else if (to_lo)
-                *reinterpret_cast<uint4*>(buf + 1024 + lane * 32 + ((c ^ sw) << 4)) =
-                    make_uint4(lw[4 * c], lw[4 * c + 1], lw[4 * c + 2], lw[4 * c + 3]);
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_3d(&tmO0, buf, n0 + c0, (int)(m_base), z);
-            if (planes && q8) {      // byte tensor map: column n sits at byte (n / 64) * 128 + n % 64 of its row, q_lo 64 further
-              const int n = n0 + c0, cb = ((n >> 6) << 7) + (n & 63);
-              tma_store_3d(&tmO1, buf + 1024, cb, (int)(m_base), z);
-              tma_store_3d(&tmO1, buf + 1536, cb + 64, (int)(m_base), z);
-            } else if (planes && to_lo) {
-              tma_store_3d(&tmO1, buf + 1024, n0 + c0, (int)(m_base), z);
-            }
-            tma_store_commit();
-          }
-          ++tma_cnt;
+        for (int h = 0; h < 2; ++h) {
+          const int rw = wi * 16 + rsub + 8 * h, cc = 8 * (j & 3) + 2 * cq;
+          const int rr = rw & 31, c16 = cc & 15;
+          float* dst = stg_wg + ((rw >> 5) | ((cc >> 4) << 1)) * 512 + rr * 16 + (((c16 >> 2) ^ ((rr >> 1) & 3)) << 2) + (c16 & 3);
+          *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
-      } else if (interior) {
-        if (p.tma_out && tma_cnt) {   // (GEGLU never sets tma_out; kept for symmetry with the edge path below)
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-        }
+      }
+      named_bar_sync(1 + wg, 128);
+      const int c0 = ch * 32 + (wi >> 1) * 16;
+      if (interior) {
         // fast path: whole tile in range, vector accesses; per-row offsets hoisted out of the column loop
-        constexpr bool EXTRA = EPI == 1, GEGLU = EPI == 2;
-        long long oD[4], oR[4], oH[4];
-        const float* rbp[4];
-        float bm[4];
+        GnAcc gacc;
+        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (has_bias) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0 + cq * 4));
+        float4 q[4];
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {
+          const int rr = it * 8 + rsub;
+          q[it] = *reinterpret_cast<const float4*>(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2));
+        }
+        const int nn = n0 + c0 + cq * 4;
+        float4 r4[4];
+        if (has_res) {
+#pragma unroll
+          for (int it = 0; it < 4; ++it)
+            r4[it] = *reinterpret_cast<const float4*>(p.res + (long long)z * p.res_bs + (long long)(m_base + it * 8 + rsub) * p.ldres + nn);
+        }
 #pragma unroll
         for (int it = 0; it < 4; ++it) {
           const long long m = m_base + it * 8 + rsub;
-          const int nn = n0 + cq * 4;
-          oD[it] = (long long)z * p.d_bs + m * p.ldd + nn;
-          oR[it] = EXTRA ? (long long)z * p.res_bs + m * p.ldres + nn : 0;
-          oH[it] = (long long)z * p.h_bs + m * p.ldh + nn;
-          rbp[it] = (EXTRA && p.rowbias)
-                        ? p.rowbias + (((long long)z * p.M + m) / p.rows_per_group) * p.rowbias_ld + nn : nullptr;
-          bm[it] = (EXTRA && p.bias_m) ? __ldg(p.bias_m + m) : 0.f;
+          float e[4] = {q[it].x, q[it].y, q[it].z, q[it].w};
+          const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
+          const float bm = (EXTRA && p.bias_m) ? __ldg(p.bias_m + m) : 0.f;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) e[j] = fmaf(e[j], alpha, EXTRA ? bb[j] + bm : bb[j]);
+          if (EXTRA && p.rowbias) {
+            const float4 rb = __ldg(reinterpret_cast<const float4*>(
+                p.rowbias + (((long long)z * p.M + m) / p.rows_per_group) * p.rowbias_ld + nn));
+            e[0] += rb.x; e[1] += rb.y; e[2] += rb.z; e[3] += rb.w;
+          }
+          if (GEGLU) {
+            // ldm GEGLU fused: lanes with even cq hold 4 `a` values, their xor-1 partner the 4 gates of the same
+            // channels (weight rows were quad-interleaved at load time); output planes have N/2 columns
+            // both partners work: the even lane finishes channels 0,1 of the quad, the odd lane channels 2,3
+            const bool odd = cq & 1;
+            const float r0 = __shfl_xor_sync(0xffffffffu, odd ? e[0] : e[2], 1);
+            const float r1 = __shfl_xor_sync(0xffffffffu, odd ? e[1] : e[3], 1);
+            const float a0 = odd ? r0 : e[0], a1 = odd ? r1 : e[1];
+            const float g0 = odd ? e[2] : r0, g1 = odd ? e[3] : r1;
+            const float gv[2] = {a0 * gelu_erf_fast(g0), a1 * gelu_erf_fast(g1)};
+            const long long og = (long long)z * p.h_bs + m * p.ldh + ((n0 + c0) >> 1) + (cq >> 1) * 4 + (odd ? 2 : 0);
+            store_planes<2>(p.Dh + og, to_lo ? p.Dl + og : nullptr, gv);
+            continue;
+          }
+          if (act != ODISE_ACT_NONE) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) e[j] = apply_act(e[j], act);
+          }
+          if (has_res) { e[0] += r4[it].x; e[1] += r4[it].y; e[2] += r4[it].z; e[3] += r4[it].w; }
+          if (has_gn) gn_acc_rows(gacc, e, it == 0, lane);
+          if (to_f32) *reinterpret_cast<float4*>(p.D + (long long)z * p.d_bs + m * p.ldd + nn) = make_float4(e[0], e[1], e[2], e[3]);
+          const long long oh = (long long)z * p.h_bs + m * p.ldh + nn;
+          if (to_hi && p.h16) {
+            // fp16 (hi, lo) planes: the V^T operand of the attention kernel's P V product
+            const __half2 h01 = __floats2half2_rn(e[0], e[1]), h23 = __floats2half2_rn(e[2], e[3]);
+            uint2 hv;
+            hv.x = *reinterpret_cast<const uint32_t*>(&h01);
+            hv.y = *reinterpret_cast<const uint32_t*>(&h23);
+            *reinterpret_cast<uint2*>(p.Dh + oh) = hv;
+            if (to_lo) {
+              const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
+              const __half2 l01 = __floats2half2_rn(e[0] - f01.x, e[1] - f01.y);
+              const __half2 l23 = __floats2half2_rn(e[2] - f23.x, e[3] - f23.y);
+              uint2 lv;
+              lv.x = *reinterpret_cast<const uint32_t*>(&l01);
+              lv.y = *reinterpret_cast<const uint32_t*>(&l23);
+              *reinterpret_cast<uint2*>(p.Dl + oh) = lv;
+            }
+          } else if (to_hi) {
+            // bf16 pair (packed conversions, same values as split_bf16) or, when Dl carries the tag, fp16 + e5m2 bytes
+            store_planes<4>(p.Dh + oh, to_lo ? p.Dl + oh : nullptr, e);
+          }
         }
-        const bool has_bias = p.bias != nullptr, has_res = EXTRA && p.res != nullptr;
-        const bool to_f32 = p.D != nullptr, to_hi = p.Dh != nullptr, to_lo = p.Dl != nullptr;
-        const int act = p.act;
-        const float alpha = p.alpha;
-        const bool has_gn = !GEGLU && p.gnp != nullptr;
-        const long long gn_seg = ((long long)z * p.M + m_base) >> 5;
+        if (has_gn) gn_acc_store(gacc, p, gn_seg, n0 + c0 + cq * 4, 4, lane);
+      } else if (n0 + c0 < p.N) {   // warp-uniform
+        // fused GroupNorm statistics on edge tiles: whole 32-row segments only (M % 32 == 0 is checked on the host)
+        const bool gn_here = p.gnp != nullptr && !p.geglu && p.splits == 1 && m_base < p.M;
+        GnAcc gacc;
 #pragma unroll 1
-        for (int c0 = c_first; c0 < BN; c0 += c_step) {
-          uint32_t v[16];
-          GnAcc gacc;
-          tmem_ld16(t_row + c0, v);
-          tmem_ld_wait();
+        for (int it = 0; it < 4; ++it) {
+          const int rr = it * 8 + rsub;
+          const float4 q4 = *reinterpret_cast<const float4*>(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2));
+          const int m = m_base + rr, n = n0 + c0 + cq * 4;
+          if (p.geglu) {   // warp-uniform; N % 16 == 0 so a chunk is either fully valid or skipped above
+            float e[4] = {q4.x, q4.y, q4.z, q4.w};
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-            *reinterpret_cast<float4*>(stg + lane * 16 + ((j ^ ((lane >> 1) & 3)) << 2)) =
-                make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]),
-                            __uint_as_float(v[4 * j + 3]));
-          __syncwarp();
-          float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (has_bias) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0 + cq * 4));
-          float4 q[4];
+            for (int j = 0; j < 4; ++j) e[j] = fmaf(e[j], p.alpha, p.bias ? __ldg(p.bias + n + j) : 0.f);
+            float gt[4];
 #pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int rr = it * 8 + rsub;
-            q[it] = *reinterpret_cast<const float4*>(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2));
+            for (int j = 0; j < 4; ++j) gt[j] = __shfl_xor_sync(0xffffffffu, e[j], 1);
+            if ((cq & 1) == 0 && m < p.M) {
+              float gv[4];
+#pragma unroll
+              for (int t = 0; t < 4; ++t) gv[t] = e[t] * gelu_erf_fast(gt[t]);
+              const long long og = (long long)z * p.h_bs + (long long)m * p.ldh + ((n0 + c0) >> 1) + (cq >> 1) * 4;
+              store_planes<4>(p.Dh + og, p.Dl ? p.Dl + og : nullptr, gv);
+            }
+            continue;
           }
-          float4 r4[4];
-          if (has_res) {
+          float fin[4] = {0.f, 0.f, 0.f, 0.f};
+          if (m < p.M && n < p.N) {
+            const int valid = min(4, p.N - n);
+            if (p.splits > 1) {
+              float* dst = p.partial + ((long long)(sp * p.batch + z) * p.M + m) * p.N + n;
+              const float e[4] = {q4.x, q4.y, q4.z, q4.w};
 #pragma unroll
-            for (int it = 0; it < 4; ++it) r4[it] = *reinterpret_cast<const float4*>(p.res + oR[it] + c0);
-          }
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            float e[4] = {q[it].x, q[it].y, q[it].z, q[it].w};
-            const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) e[j] = fmaf(e[j], alpha, EXTRA ? bb[j] + bm[it] : bb[j]);
-            if (EXTRA && rbp[it]) {
-              const float4 rb = __ldg(reinterpret_cast<const float4*>(rbp[it] + c0));
-              e[0] += rb.x; e[1] += rb.y; e[2] += rb.z; e[3] += rb.w;
-            }
-            if (GEGLU) {
-              // ldm GEGLU fused: lanes with even cq hold 4 `a` values, their xor-1 partner the 4 gates of the same
-              // channels (weight rows were quad-interleaved at load time); output planes have N/2 columns
-              // both partners work: the even lane finishes channels 0,1 of the quad, the odd lane channels 2,3
-              const bool odd = cq & 1;
-              const float r0 = __shfl_xor_sync(0xffffffffu, odd ? e[0] : e[2], 1);
-              const float r1 = __shfl_xor_sync(0xffffffffu, odd ? e[1] : e[3], 1);
-              const float a0 = odd ? r0 : e[0], a1 = odd ? r1 : e[1];
-              const float g0 = odd ? e[2] : r0, g1 = odd ? e[3] : r1;
-              const float gv[2] = {a0 * gelu_erf_fast(g0), a1 * gelu_erf_fast(g1)};
-              const long long og = (long long)z * p.h_bs + (long long)(m_base + it * 8 + rsub) * p.ldh +
-                                   ((n0 + c0) >> 1) + (cq >> 1) * 4 + (odd ? 2 : 0);
-              store_planes<2>(p.Dh + og, to_lo ? p.Dl + og : nullptr, gv);
-              continue;
-            }
-            if (act != ODISE_ACT_NONE) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) e[j] = apply_act(e[j], act);
-            }
-            if (has_res) { e[0] += r4[it].x; e[1] += r4[it].y; e[2] += r4[it].z; e[3] += r4[it].w; }
-            if (has_gn) gn_acc_rows(gacc, e, it == 0, lane);
-            if (to_f32) *reinterpret_cast<float4*>(p.D + oD[it] + c0) = make_float4(e[0], e[1], e[2], e[3]);
-            if (to_hi && p.h16) {
-              // fp16 (hi, lo) planes: the V^T operand of the attention kernel's P V product
-              const __half2 h01 = __floats2half2_rn(e[0], e[1]), h23 = __floats2half2_rn(e[2], e[3]);
-              uint2 hv;
-              hv.x = *reinterpret_cast<const uint32_t*>(&h01);
-              hv.y = *reinterpret_cast<const uint32_t*>(&h23);
-              *reinterpret_cast<uint2*>(p.Dh + oH[it] + c0) = hv;
-              if (to_lo) {
-                const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-                const __half2 l01 = __floats2half2_rn(e[0] - f01.x, e[1] - f01.y);
-                const __half2 l23 = __floats2half2_rn(e[2] - f23.x, e[3] - f23.y);
-                uint2 lv;
-                lv.x = *reinterpret_cast<const uint32_t*>(&l01);
-                lv.y = *reinterpret_cast<const uint32_t*>(&l23);
-                *reinterpret_cast<uint2*>(p.Dl + oH[it] + c0) = lv;
-              }
-            } else if (to_hi) {
-              // bf16 pair (packed conversions, same values as split_bf16) or, when Dl carries the tag, fp16 + e5m2 bytes
-              store_planes<4>(p.Dh + oH[it] + c0, to_lo ? p.Dl + oH[it] + c0 : nullptr, e);
+              for (int j = 0; j < 4; ++j) if (j < valid) dst[j] = e[j];
+            } else {
+              epilogue_quad(p, z, m, n, valid, q4, fin);
             }
           }
-          if (has_gn) gn_acc_store(gacc, p, gn_seg, n0 + c0 + cq * 4, 4, lane);
-          __syncwarp();
+          if (gn_here) gn_acc_rows(gacc, fin, it == 0, lane);      // warp-uniform: all lanes shuffle
         }
-      } else {
-        if (p.tma_out && tma_cnt) {   // an edge tile reuses the staging buffer with plain stores: drain the TMA reads first
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-        }
-#pragma unroll 1
-        for (int c0 = c_first; c0 < BN; c0 += c_step) {
-          uint32_t v[16];
-          tmem_ld16(t_row + c0, v);
-          tmem_ld_wait();
-          if (n0 + c0 < p.N) {   // warp-uniform
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float4 q4 = has_k ? make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                    __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]))
-                                      : make_float4(0.f, 0.f, 0.f, 0.f);
-              *reinterpret_cast<float4*>(stg + lane * 16 + ((j ^ ((lane >> 1) & 3)) << 2)) = q4;
-            }
-            __syncwarp();
-            // fused GroupNorm statistics on edge tiles: whole 32-row segments only (M % 32 == 0 is checked on the host)
-            const bool gn_here = p.gnp != nullptr && !p.geglu && p.splits == 1 && m_base < p.M;
-            GnAcc gacc;
-#pragma unroll 1
-            for (int it = 0; it < 4; ++it) {
-              const int rr = it * 8 + rsub;
-              const float4 q4 = *reinterpret_cast<const float4*>(stg + rr * 16 + ((cq ^ ((rr >> 1) & 3)) << 2));
-              const int m = m_base + rr, n = n0 + c0 + cq * 4;
-              if (p.geglu) {   // warp-uniform; N % 16 == 0 so a chunk is either fully valid or skipped above
-                float e[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) e[j] = fmaf(e[j], p.alpha, p.bias ? __ldg(p.bias + n + j) : 0.f);
-                float gt[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) gt[j] = __shfl_xor_sync(0xffffffffu, e[j], 1);
-                if ((cq & 1) == 0 && m < p.M) {
-                  float gv[4];
-#pragma unroll
-                  for (int t = 0; t < 4; ++t) gv[t] = e[t] * gelu_erf_fast(gt[t]);
-                  const long long og = (long long)z * p.h_bs + (long long)m * p.ldh + ((n0 + c0) >> 1) + (cq >> 1) * 4;
-                  store_planes<4>(p.Dh + og, p.Dl ? p.Dl + og : nullptr, gv);
-                }
-                continue;
-              }
-              float fin[4] = {0.f, 0.f, 0.f, 0.f};
-              if (m < p.M && n < p.N) {
-                const int valid = min(4, p.N - n);
-                if (p.splits > 1) {
-                  float* dst = p.partial + ((long long)(sp * p.batch + z) * p.M + m) * p.N + n;
-                  const float e[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) if (j < valid) dst[j] = e[j];
-                } else {
-                  epilogue_quad(p, z, m, n, valid, q4, fin);
-                }
-              }
-              if (gn_here) gn_acc_rows(gacc, fin, it == 0, lane);      // warp-uniform: all lanes shuffle
-            }
-            if (gn_here) {
-              const int n = n0 + c0 + cq * 4;
-              gn_acc_store(gacc, p, ((long long)z * p.M + m_base) >> 5, n, n < p.N ? min(4, p.N - n) : 0, lane);
-            }
-            __syncwarp();
-          }
+        if (gn_here) {
+          const int n = n0 + c0 + cq * 4;
+          gn_acc_store(gacc, p, ((long long)z * p.M + m_base) >> 5, n, n < p.N ? min(4, p.N - n) : 0, lane);
         }
       }
-      tc_fence_before();
-      if (SM2 && crank == 1) mbar_arrive_remote(mapa_shared(&tempty[acc], 0));   // the pair's accumulator belongs to the leader's MMA thread
-      else mbar_arrive(&tempty[acc]);
-      if (++acc == 2) { acc = 0; accphase ^= 1; }
     }
-    if (p.tma_out && lane == 0 && tma_cnt) tma_store_wait_read<0>();   // shared memory must outlive the stores' reads
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (p.cl > 1) cluster_sync();        // no CTA leaves while its peer can still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    if (SM2) tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-    else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
@@ -854,38 +613,8 @@ static int encode_map(CUtensorMap* tm, const void* base, int rank, const cuuint6
   return r == CUDA_SUCCESS ? ODISE_OK : ODISE_ERR_TENSORMAP;
 }
 
-// output tensor map of the TMA-store epilogue: {N, M, batch}, box {16 columns, 32 rows, 1}; fp32 rows of the box are 64 B
-// (SWIZZLE_64B), 16-bit plane rows 32 B (SWIZZLE_32B) — the staging writes in the kernel use the same XOR patterns
-// second plane of F16Q8 output planes as bytes: {2 * ld bytes, M, batch}, box {16 bytes, 32 rows, 1}, no swizzle
-static int encode_q8_out_map(CUtensorMap* tm, void* base, long long M, long long batch, long long ld, long long bs) {
-  auto enc = get_encode();
-  if (!enc) return ODISE_ERR_DRIVER;
-  cuuint64_t dims[3] = {(cuuint64_t)ld * 2, (cuuint64_t)M, (cuuint64_t)batch};
-  cuuint64_t str[2] = {(cuuint64_t)ld * 2, (cuuint64_t)(batch > 1 ? bs : M * ld) * 2};
-  cuuint32_t box[3] = {16, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, base, dims, str, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? ODISE_OK : ODISE_ERR_TENSORMAP;
-}
-
-static int encode_out_map(CUtensorMap* tm, void* base, bool f32, long long N, long long M, long long batch, long long ld,
-                          long long bs) {
-  auto enc = get_encode();
-  if (!enc) return ODISE_ERR_DRIVER;
-  const cuuint64_t es = f32 ? 4 : 2;
-  cuuint64_t dims[3] = {(cuuint64_t)N, (cuuint64_t)M, (cuuint64_t)batch};
-  cuuint64_t str[2] = {(cuuint64_t)ld * es, (cuuint64_t)(batch > 1 ? bs : M * ld) * es};
-  cuuint32_t box[3] = {16, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, base, dims, str, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, f32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B,
-                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? ODISE_OK : ODISE_ERR_TENSORMAP;
-}
-
 // ---- optional per-launch timing (bench.py roofline): CUDA events on the launch stream around every GEMM launch
-struct ProfRec { cudaEvent_t a, b; double flops; int M, N, K, batch, conv, bn, nmma, splits, pair; };
+struct ProfRec { cudaEvent_t a, b; double flops; int M, N, K, batch, conv, bn, nmma, splits; };
 static std::vector<ProfRec> g_prof;
 static bool g_prof_on = false;
 
@@ -895,88 +624,53 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-template <int BN, int NMMA, int EPI, int SM2>
+template <int BN, int NMMA, int EPI>
 static int launch_cfg(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                      const CUtensorMap& o0, const CUtensorMap& o1, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, NMMA, SM2>;
+                      const GemmParams& p, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN, NMMA>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, NMMA, EPI, SM2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, NMMA, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return (int)e;
     attr_set = true;
   }
-  const int total = p.tiles_mp * p.tiles_n * p.splits * p.batch;       // tiles (cl = 1) or pairs of M tiles (cl = 2)
-  if (p.cl == 1) {
-    const int grid = total < num_sms() ? total : num_sms();
-    gemm_tc_kernel<BN, NMMA, EPI, SM2><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(ah, al, bh, bl, o0, o1, p);
-    return (int)cudaGetLastError();
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(Cfg::THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  // a persistent grid must be ONE resident wave: pairs are placed inside a GPC, and a GPC with an odd number of usable SMs
-  // leaves one idle -> ask the driver how many 2-CTA clusters of this kernel can be co-resident
-  static int max_pairs = 0;
-  if (!max_pairs) {
-    cfg.gridDim = dim3(2 * (num_sms() / 2));
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, gemm_tc_kernel<BN, NMMA, EPI, SM2>, &cfg) != cudaSuccess || n <= 0) {
-      (void)cudaGetLastError();
-      n = num_sms() / 2 - 4;
-    }
-    max_pairs = n < num_sms() / 2 ? n : num_sms() / 2;
-    if (getenv("ODISE_VERBOSE")) fprintf(stderr, "odise_b200: gemm_tc<%d,%d,%d,%d> co-resident CTA pairs: %d\n", BN, NMMA, EPI, SM2, max_pairs);
-  }
-  cfg.gridDim = dim3(2 * (total < max_pairs ? total : max_pairs));
-  return (int)cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, NMMA, EPI, SM2>, ah, al, bh, bl, o0, o1, p);
+  const int total = p.tiles_m * p.tiles_n * p.splits * p.batch;
+  const int grid = total < num_sms() ? total : num_sms();
+  gemm_tc_kernel<BN, NMMA, EPI><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(ah, al, bh, bl, p);
+  return (int)cudaGetLastError();
 }
 
-// Tile choice: output-tile width BN and whether CTA pairs run 2-SM MMAs (GemmCfg SM2; BN = 256 only: with 64 / 80-row B
-// halves the pair MMA runs at about half rate, tools/r2_gpu_batch7.sh).  Relative time per (output column x k) of a 128-row
-// tile, measured on B200 with tools/gemm_one.py at K >= 1024 (profiles/r2j_gemm_sm2_policy.txt):
-//                       BN = 256 pair   256    160    128    64
-//   F16Q8  (nmma 2)          0.92       1.12   0.95   1.00   1.45     (two 96 KB stages starve the single-CTA 256 tile)
-//   bf16x3 (nmma 3)          0.90       1.05   0.95   1.00   1.45
-//   bf16   (nmma 1)           -         0.90   0.95   1.00   1.45
-struct TileChoice { int bn; bool sm2; };
-static TileChoice pick_tile(int M, int N, int K, int batch, int forced, bool conv, int nmma, bool pair_ok) {
-  const int cands[5] = {256, 256, 160, 128, 64};                 // cands[0] = the pair variant
-  const double eff2[5] = {0.92, 1.12, 0.95, 1.0, 1.45}, eff3[5] = {0.90, 1.05, 0.95, 1.0, 1.45},
-               eff1[5] = {9.9, 0.90, 0.95, 1.0, 1.45};
-  const double* eff = nmma == 2 ? eff2 : (nmma == 3 ? eff3 : eff1);
-  const double epi_k[5] = {480.0, 480.0, 960.0, 480.0, 480.0};  // epilogue of a tile in units of MMA k (8 / 4 epilogue warps)
+// Tile choice: output-tile width BN.  eff = shared-memory operand bytes per MAC of a warpgroup's 64 x BN wgmma tile
+// ((64 + BN) / (64 BN)), relative to BN = 128: wider tiles re-read A less often.  The per-shape autotune in
+// odise_gemm_bf16 replaces this estimate wherever it may launch trial runs.
+static int pick_tile(int M, int N, int K, int batch, int forced, bool conv, int nmma) {
+  const int cands[4] = {256, 160, 128, 64};
+  const double eff[4] = {0.833, 0.933, 1.0, 1.333};
+  const double epi_k = 480.0;    // epilogue of a tile in units of MMA k
   const long long tm = (M + 127) / 128;
   double best = 1e30;
-  TileChoice c{128, false};
-  for (int i = 0; i < 5; ++i) {
+  int c = 128;
+  for (int i = 0; i < 4; ++i) {
     const int bn = cands[i];
-    const bool sm2 = i == 0;
-    if (sm2 && !(pair_ok && nmma != 1 && K >= 1024)) continue;
     if (forced && bn != forced) continue;
+    if (nmma == 2 && bn > 128) continue;
     const long long tn = (N + bn - 1) / bn;
-    const long long units = sm2 ? ((tm + 1) / 2) * tn * batch : tm * tn * batch;
-    const long long slots = sm2 ? num_sms() / 2 : num_sms();
-    const long long waves = (units + slots - 1) / slots;
+    const long long units = tm * tn * batch;
+    const long long waves = (units + num_sms() - 1) / num_sms();
     double cost;
     if (conv) {          // implicit convs (K >= 576): main-loop bound at every width -> balance waves
       cost = (double)waves * bn * eff[i] + 0.02 * bn;            // mild bias toward smaller tiles on ties
     } else {             // plain GEMMs: per-tile time = max(main loop, epilogue) + fixed fill / drain
-      const double mma = (double)bn * K * eff[i], epi = (double)bn * epi_k[i];
+      const double mma = (double)bn * K * eff[i], epi = (double)bn * epi_k;
       cost = (double)waves * ((mma > epi ? mma : epi) + 20000.0);
     }
-    if (cost < best) { best = cost; c = TileChoice{bn, sm2}; }
+    if (cost < best) { best = cost; c = bn; }
   }
   return c;
 }
@@ -1112,51 +806,23 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
     p.partial = reinterpret_cast<float*>(d->workspace);
   }
   const int epi = d->geglu ? 2 : ((d->residual || d->rowbias || d->bias_m) ? 1 : 0);
-  // TMA-store epilogue: one kind of output (fp32 OR planes), final values produced by this kernel, no fused GN records
-  // (those need the column-major view of the transposing epilogue).  ODISE_NO_TMA_STORE=1 keeps the round-1 epilogue (A/B).
-  CUtensorMap o0 = ah, o1 = ah;
-  {
-    static const bool off = getenv("ODISE_NO_TMA_STORE") != nullptr;
-    const bool one_kind = (d->out_f32 != nullptr) != (d->out_hi != nullptr);
-    if (!off && epi != 2 && p.vec_ok && p.splits == 1 && !p.gnp && one_kind) {
-      if (d->out_f32) {
-        rc = encode_out_map(&o0, d->out_f32, true, d->N, d->M, d->batch, d->ld_out, d->out_batch_stride);
-        if (!rc) p.tma_out = 1;
-      } else {
-        rc = encode_out_map(&o0, d->out_hi, false, d->N, d->M, d->batch, d->ld_out_bf16, d->out_bf16_batch_stride);
-        if (!rc && oq8)
-          rc = encode_q8_out_map(&o1, d->out_lo, d->M, d->batch, d->ld_out_bf16, d->out_bf16_batch_stride);
-        else if (!rc && d->out_lo)
-          rc = encode_out_map(&o1, d->out_lo, false, d->N, d->M, d->batch, d->ld_out_bf16, d->out_bf16_batch_stride);
-        if (!rc) p.tma_out = 2;
-      }
-      if (rc) p.tma_out = 0;      // a shape the tensor map cannot express: the plain epilogue handles it
-    }
-  }
 
-  // one launch with a given output-tile width / pairing: B tensor maps (box = bn rows, bn / 2 per CTA of a pair) + dispatch
-  auto launch_with = [&](int bn, int cl, bool s2) -> int {
-    p.cl = cl;
-    p.tiles_mp = (p.tiles_m + cl - 1) / cl;
+  // one launch with a given output-tile width: B tensor map (box = bn rows) + dispatch
+  auto launch_with = [&](int bn) -> int {
     p.tiles_n = (d->N + bn - 1) / bn;
     const long long bs = d->b_batch_stride ? d->b_batch_stride : (long long)d->N * d->ldb;
     cuuint64_t dims[3] = {(cuuint64_t)d->K, (cuuint64_t)d->N, (cuuint64_t)(d->b_batch_stride ? d->batch : 1)};
     cuuint64_t str[2] = {(cuuint64_t)d->ldb * 2, (cuuint64_t)bs * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)(bn / cl), 1};     // pair modes: each CTA fetches half of the B tile
+    cuuint32_t box[3] = {64, (cuuint32_t)bn, 1};
     int r = encode_map(&bh, d->b_hi, 3, dims, str, box);
     if (r) return r;
     if (d->nmma == 2) dims[0] = (cuuint64_t)((d->K + 63) / 64 * 64);   // whole 64-blocks of q bytes
     r = encode_map(&bl, d->nmma != 1 ? d->b_lo : d->b_hi, 3, dims, str, box);
     if (r) return r;
-#define ODISE_LAUNCH_E(BN_, NM_, S_)                                                  \
-  r = epi == 2   ? launch_cfg<BN_, NM_, 2, S_>(ah, al, bh, bl, o0, o1, p, stream)     \
-      : epi == 1 ? launch_cfg<BN_, NM_, 1, S_>(ah, al, bh, bl, o0, o1, p, stream)     \
-                 : launch_cfg<BN_, NM_, 0, S_>(ah, al, bh, bl, o0, o1, p, stream)
-#define ODISE_LAUNCH(BN_, NM_)                                                        \
-  do {                                                                                \
-    if (s2 && NM_ != 1) { ODISE_LAUNCH_E(BN_, (NM_ == 1 ? 3 : NM_), 1); }             \
-    else { ODISE_LAUNCH_E(BN_, NM_, 0); }                                             \
-  } while (0)
+#define ODISE_LAUNCH(BN_, NM_)                                                   \
+  r = epi == 2   ? launch_cfg<BN_, NM_, 2>(ah, al, bh, bl, p, stream)            \
+      : epi == 1 ? launch_cfg<BN_, NM_, 1>(ah, al, bh, bl, p, stream)            \
+                 : launch_cfg<BN_, NM_, 0>(ah, al, bh, bl, p, stream)
     if (d->nmma == 3) {
       switch (bn) {
         case 64: ODISE_LAUNCH(64, 3); break;
@@ -1165,12 +831,8 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
         default: ODISE_LAUNCH(256, 3); break;
       }
     } else if (d->nmma == 2) {
-      switch (bn) {
-        case 64: ODISE_LAUNCH(64, 2); break;
-        case 128: ODISE_LAUNCH(128, 2); break;
-        case 160: ODISE_LAUNCH(160, 2); break;
-        default: ODISE_LAUNCH(256, 2); break;
-      }
+      if (bn == 64) ODISE_LAUNCH(64, 2);
+      else ODISE_LAUNCH(128, 2);
     } else {
       switch (bn) {
         case 64: ODISE_LAUNCH(64, 1); break;
@@ -1180,86 +842,70 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
       }
     }
 #undef ODISE_LAUNCH
-#undef ODISE_LAUNCH_E
     if (r) return r;
     if (p.splits > 1) {
       const long long total = (long long)p.batch * p.M * ((p.N + 3) / 4);
       int blocks = (int)((total + 127) / 128);
-      if (blocks > 148 * 8) blocks = 148 * 8;
+      if (blocks > num_sms() * 8) blocks = num_sms() * 8;
       gemm_splitk_reduce_kernel<<<blocks, 128, 0, stream>>>(p);
       r = (int)cudaGetLastError();
     }
     return r;
   };
 
-  // ---- tile width / pairing.  ODISE_GEMM_CLUSTER: 1 (default) = measured choice: a per-shape autotune (every candidate is
-  // the same arithmetic in the same k order -> bit-identical results, so the choice is free) with the cost model
-  // pick_tile() as the fallback under stream capture; 0 = single CTAs; 2 = 2-SM MMAs wherever there are two M tiles;
-  // 3 / 4 = 1-SM MMAs + multicast B pairs (A/B switches).  ODISE_GEMM_AUTOTUNE=0: cost model only.
-  bool sm2 = false;
-  int BN, CL = 1;
+  // ---- tile width: a per-shape autotune (every candidate is the same arithmetic in the same k order -> bit-identical
+  // results, so the choice is free) with the cost model pick_tile() as the fallback under stream capture.
+  // ODISE_GEMM_AUTOTUNE=0: cost model only.
+  int BN;
   {
-    static const int mode = getenv("ODISE_GEMM_CLUSTER") ? atoi(getenv("ODISE_GEMM_CLUSTER")) : 1;
     static const bool tune = !(getenv("ODISE_GEMM_AUTOTUNE") && atoi(getenv("ODISE_GEMM_AUTOTUNE")) == 0);
-    const bool pairable = p.tiles_m >= 2 && (p.tiles_m % 2 == 0 || p.tiles_m >= 16);
     const int fbn = (d->force_bn == 64 || d->force_bn == 128 || d->force_bn == 160 || d->force_bn == 256) ? d->force_bn : 0;
-    if (mode != 1) {
-      BN = pick_tile(d->M, d->N, d->K, d->batch, fbn, d->conv3x3 != 0, d->nmma, false).bn;
-      if ((mode == 2 || mode == 4) && p.tiles_m >= 2) CL = 2;
-      else if (mode == 3 && pairable) CL = 2;
-      sm2 = CL == 2 && mode == 2 && d->nmma != 1;
-    } else {
-      const TileChoice tc = pick_tile(d->M, d->N, d->K, d->batch, fbn, d->conv3x3 != 0, d->nmma, pairable);
-      BN = tc.bn; sm2 = tc.sm2;
-      struct Key {
-        int v[14];
-        bool operator<(const Key& o) const { return memcmp(v, o.v, sizeof(v)) < 0; }
-      };
-      static std::map<Key, TileChoice> cache;
-      static std::mutex mu;
-      const Key key{{d->M, d->N, d->K, d->batch, d->conv3x3 ? 1 + d->conv_mode : 0, d->conv_W, d->nmma, epi, p.splits,
-                    (d->out_f32 ? 1 : 0) | (d->out_hi ? 2 : 0) | (d->out_planes_fp16 << 2), p.gnp ? 1 : 0, d->act, p.tma_out,
-                    p.vec_ok}};
-      cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-      cudaStreamIsCapturing(stream, &cap);
-      std::lock_guard<std::mutex> lk(mu);
-      auto it = cache.find(key);
-      if (it != cache.end()) {
-        BN = it->second.bn; sm2 = it->second.sm2;
-      } else if (tune && !fbn && !g_prof_on && cap == cudaStreamCaptureStatusNone &&
-                 !(d->residual && (const void*)d->residual == (const void*)d->out_f32)) {
-        // candidates: the pair tile, then single CTAs from wide to narrow (64 only for narrow outputs)
-        const TileChoice cands[5] = {{256, true}, {256, false}, {160, false}, {128, false}, {64, false}};
-        cudaEvent_t e0, e1;
-        cudaEventCreate(&e0);
-        cudaEventCreate(&e1);
-        float best = 1e30f;
-        TileChoice bc = tc;
-        for (int i = 0; i < 5; ++i) {
-          const TileChoice c = cands[i];
-          if (c.sm2 && !(pairable && d->nmma != 1)) continue;
-          // 64-wide tiles: narrow outputs, or problems too small to fill the SMs with wider ones (decoder linears)
-          if (c.bn == 64 && d->N > 96 && (long long)p.tiles_m * ((d->N + 127) / 128) * d->batch >= 2 * num_sms()) continue;
-          if (c.bn > 128 && d->N <= 64) continue;
-          if (launch_with(c.bn, c.sm2 ? 2 : 1, c.sm2)) { (void)cudaGetLastError(); continue; }     // warm (attributes, L2)
-          cudaEventRecord(e0, stream);
-          int r2 = launch_with(c.bn, c.sm2 ? 2 : 1, c.sm2);
-          if (!r2) r2 = launch_with(c.bn, c.sm2 ? 2 : 1, c.sm2);
-          cudaEventRecord(e1, stream);
-          if (r2 || cudaEventSynchronize(e1) != cudaSuccess) { (void)cudaGetLastError(); continue; }
-          float ms = 0.f;
-          cudaEventElapsedTime(&ms, e0, e1);
-          if (ms < best) { best = ms; bc = c; }
-        }
-        cudaEventDestroy(e0);
-        cudaEventDestroy(e1);
-        cache[key] = bc;
-        BN = bc.bn; sm2 = bc.sm2;
-        if (getenv("ODISE_VERBOSE"))
-          fprintf(stderr, "odise_b200: gemm %d x %d x %d (batch %d, conv %d, nmma %d, epi %d): BN %d%s, %.1f us\n", d->M, d->N,
-                  d->K, d->batch, d->conv3x3, d->nmma, epi, BN, sm2 ? " pair (2-SM MMAs)" : "", best * 500.f);
+    BN = pick_tile(d->M, d->N, d->K, d->batch, fbn, d->conv3x3 != 0, d->nmma);
+    struct Key {
+      int v[13];
+      bool operator<(const Key& o) const { return memcmp(v, o.v, sizeof(v)) < 0; }
+    };
+    static std::map<Key, int> cache;
+    static std::mutex mu;
+    const Key key{{d->M, d->N, d->K, d->batch, d->conv3x3 ? 1 + d->conv_mode : 0, d->conv_W, d->nmma, epi, p.splits,
+                  (d->out_f32 ? 1 : 0) | (d->out_hi ? 2 : 0) | (d->out_planes_fp16 << 2), p.gnp ? 1 : 0, d->act, p.vec_ok}};
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(stream, &cap);
+    std::lock_guard<std::mutex> lk(mu);
+    auto it = cache.find(key);
+    if (it != cache.end()) {
+      BN = it->second;
+    } else if (tune && !fbn && !g_prof_on && cap == cudaStreamCaptureStatusNone &&
+               !(d->residual && (const void*)d->residual == (const void*)d->out_f32)) {
+      // candidates from wide to narrow (64 only for narrow outputs)
+      const int cands[4] = {256, 160, 128, 64};
+      cudaEvent_t e0, e1;
+      cudaEventCreate(&e0);
+      cudaEventCreate(&e1);
+      float best = 1e30f;
+      int bc = BN;
+      for (int i = 0; i < 4; ++i) {
+        const int c = cands[i];
+        // 64-wide tiles: narrow outputs, or problems too small to fill the SMs with wider ones (decoder linears)
+        if (c == 64 && d->N > 96 && (long long)p.tiles_m * ((d->N + 127) / 128) * d->batch >= 2 * num_sms()) continue;
+        if (c > 128 && (d->N <= 64 || d->nmma == 2)) continue;
+        if (launch_with(c)) { (void)cudaGetLastError(); continue; }     // warm (attributes, L2)
+        cudaEventRecord(e0, stream);
+        int r2 = launch_with(c);
+        if (!r2) r2 = launch_with(c);
+        cudaEventRecord(e1, stream);
+        if (r2 || cudaEventSynchronize(e1) != cudaSuccess) { (void)cudaGetLastError(); continue; }
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, e0, e1);
+        if (ms < best) { best = ms; bc = c; }
       }
-      if (sm2) CL = 2;
+      cudaEventDestroy(e0);
+      cudaEventDestroy(e1);
+      cache[key] = bc;
+      BN = bc;
+      if (getenv("ODISE_VERBOSE"))
+        fprintf(stderr, "odise_b200: gemm %d x %d x %d (batch %d, conv %d, nmma %d, epi %d): BN %d, %.1f us\n", d->M, d->N,
+                d->K, d->batch, d->conv3x3, d->nmma, epi, BN, best * 500.f);
     }
   }
 
@@ -1269,10 +915,10 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
     cudaEventCreate(&rec.b);
     rec.flops = 2.0 * d->M * d->N * (double)d->K * d->batch;
     rec.M = d->M; rec.N = d->N; rec.K = d->K; rec.batch = d->batch; rec.conv = d->conv3x3; rec.bn = BN;
-    rec.nmma = d->nmma; rec.splits = p.splits; rec.pair = sm2 ? 2 : (CL == 2 ? 1 : 0);
+    rec.nmma = d->nmma; rec.splits = p.splits;
     cudaEventRecord(rec.a, stream);
   }
-  rc = launch_with(BN, CL, sm2);
+  rc = launch_with(BN);
   if (rc) return rc;
   count_launch(p.splits > 1 ? 2 : 1);
   if (g_prof_on) {
@@ -1283,14 +929,12 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
 }
 
 // The cost-model choice of odise_gemm_bf16 for a problem (what it uses under stream capture / with ODISE_GEMM_AUTOTUNE=0, and
-// the starting point of the per-shape autotune): output-tile width and whether CTA pairs run 2-SM MMAs.  Host only.
+// the starting point of the per-shape autotune): the output-tile width.  *pair reports CTA pairs, which the sm_90a kernel
+// does not use (always 0).  Host only.
 extern "C" int odise_gemm_tile_policy(int M, int N, int K, int batch, int conv3x3, int nmma, int* bn, int* pair) {
   if (M <= 0 || N <= 0 || K <= 0 || batch <= 0 || !bn || !pair || nmma < 1 || nmma > 3) return ODISE_ERR_ARG;
-  const int tiles_m = (M + 127) / 128;
-  const bool pairable = tiles_m >= 2 && (tiles_m % 2 == 0 || tiles_m >= 16);
-  const TileChoice c = pick_tile(M, N, K, batch, 0, conv3x3 != 0, nmma, pairable);
-  *bn = c.bn;
-  *pair = c.sm2 ? 1 : 0;
+  *bn = pick_tile(M, N, K, batch, 0, conv3x3 != 0, nmma);
+  *pair = 0;
   return ODISE_OK;
 }
 
@@ -1310,15 +954,15 @@ extern "C" int odise_profile_end(long long* launches, double* total_ms, double* 
   double ms = 0, fl = 0;
   FILE* fcsv = nullptr;
   if (const char* path = getenv("ODISE_PROFILE_CSV")) fcsv = fopen(path, "a");
-  if (fcsv) fprintf(fcsv, "M,N,K,batch,conv,bn,nmma,splits,ms,tflops,pair\n");   // pair: 0 single CTAs, 1 multicast pairs, 2 2-SM MMAs
+  if (fcsv) fprintf(fcsv, "M,N,K,batch,conv,bn,nmma,splits,ms,tflops\n");
   for (auto& r : g_prof) {
     float t = 0;
     cudaEventElapsedTime(&t, r.a, r.b);
     ms += t;
     fl += r.flops;
     if (fcsv)
-      fprintf(fcsv, "%d,%d,%d,%d,%d,%d,%d,%d,%.4f,%.1f,%d\n", r.M, r.N, r.K, r.batch, r.conv, r.bn, r.nmma, r.splits, t,
-              r.flops / (t * 1e9), r.pair);
+      fprintf(fcsv, "%d,%d,%d,%d,%d,%d,%d,%d,%.4f,%.1f\n", r.M, r.N, r.K, r.batch, r.conv, r.bn, r.nmma, r.splits, t,
+              r.flops / (t * 1e9));
   }
   if (fcsv) fclose(fcsv);
   if (launches) *launches = (long long)g_prof.size();

@@ -1,4 +1,4 @@
-// MaskCLIP front-end and the open-vocabulary class merge of ODISE inference (SURVEY.md §8a row b13, §8f-2), sm_100a.
+// MaskCLIP front-end and the open-vocabulary class merge of ODISE inference (SURVEY.md §8a row b13, §8f-2), sm_90a.
 //
 // Reference: MaskCLIP.get_mask_embed / encode_image_with_mask (odise/modeling/meta_arch/clip.py:284-339) resizes the
 // [0,1] image and the Q mask logits bilinearly to the CLIP resolution, max-pools sigmoid(mask) per 14x14 patch and

@@ -1,4 +1,4 @@
-// Multi-scale deformable attention sampling for sm_100a (SURVEY.md §8a rows b4/b5).
+// Multi-scale deformable attention sampling for sm_90a (SURVEY.md §8a rows b4/b5).
 //
 // Semantics follow ms_deformable_im2col_gpu_kernel / ms_deform_attn_im2col_bilinear of the reference
 // (third_party/Mask2Former/mask2former/modeling/pixel_decoder/ops/src/cuda/ms_deform_im2col_cuda.cuh:38-89,
@@ -290,7 +290,7 @@ extern "C" int odise_msda_forward_f32(const float* value, const int64_t* spatial
   } else {
     const long long total = (long long)N * Lq * M * D;
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
     msda_scalar_kernel<<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
   }
   count_launch(1);

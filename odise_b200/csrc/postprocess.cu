@@ -1,4 +1,4 @@
-// GPU post-processing of ODISE / Mask2Former inference (SURVEY.md §8a rows b13 / b14, §8f-3), sm_100a.
+// GPU post-processing of ODISE / Mask2Former inference (SURVEY.md §8a rows b13 / b14, §8f-3), sm_90a.
 //
 // Reference: CategoryODISE.forward tail (odise/modeling/meta_arch/odise.py:326-370: F.interpolate of the mask logits to
 // the padded image size, then per image semantic / panoptic / instance inference) and
@@ -530,13 +530,13 @@ extern "C" int odise_panoptic_inference_f32(const float* logits, const float* sc
   cudaError_t e = cudaMemsetAsync(counters, 0, sizeof(int32_t) * 3 * B * Q, st);
   if (e != cudaSuccess) return (int)e;
   int blocks = (int)(((long long)H * W + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
   panoptic_argmax_kernel<<<dim3(blocks, B), 256, 3 * Q * sizeof(int32_t), st>>>(logits, scores, keep, ids, fg, area, orig,
                                                                             inter, Q, H, W, make_sampler(hs, ws_, H, W, geom));
   panoptic_assign_kernel<<<B, 32, K * sizeof(int32_t), st>>>(keep, labels, area, orig, inter, is_thing, seg_of, seg_info,
                                                           n_segments, Q, K, overlap_thr);
   int rb = (int)((npix + 255) / 256);
-  if (rb > 148 * 8) rb = 148 * 8;
+  if (rb > num_sms() * 8) rb = num_sms() * 8;
   panoptic_relabel_kernel<<<rb, 256, 0, st>>>(ids, fg, seg_of, pan, Q, (long long)H * W, B);
   count_launch(3);
   return (int)cudaGetLastError();
@@ -630,7 +630,7 @@ extern "C" int odise_postprocess_fused_f32(const float* logits, void* sem_hi, vo
     panoptic_assign_kernel<<<B, 32, K * sizeof(int32_t), st>>>(keep, labels, a.area, a.orig, a.inter, is_thing, seg_of,
                                                             seg_info, n_segments, Q, K, overlap_thr);
     int rb = (int)((npix + 255) / 256);
-    if (rb > 148 * 8) rb = 148 * 8;
+    if (rb > num_sms() * 8) rb = num_sms() * 8;
     panoptic_relabel_kernel<<<rb, 256, 0, st>>>(a.ids, a.fg, seg_of, pan, Q, (long long)H * W, B);
     launches += 2;
   }

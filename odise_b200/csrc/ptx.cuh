@@ -1,6 +1,6 @@
-// Blackwell (sm_100a) PTX wrappers shared by every kernel TU: mbarrier, TMA, tcgen05/TMEM.
-// Nothing here is ported from the reference (which has no sm_90/sm_100 code at all, SURVEY.md §2.4);
-// bit layouts follow the PTX ISA as restated in the vendored CuTe headers (mma_sm100_desc.hpp).
+// Hopper (sm_90a) PTX wrappers shared by every kernel TU: mbarrier, TMA, wgmma.
+// Nothing here is ported from the reference (which has no sm_90 code at all, SURVEY.md §2.4);
+// bit layouts follow the PTX ISA (wgmma matrix descriptors, tensor-map swizzle modes).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -32,10 +32,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() {
-  // generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
@@ -54,17 +50,24 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug must abort the kernel (trap -> launch error), never hang the box.
+// Bounded wait: a pipeline bug must abort the kernel (trap -> launch error), never hang the box.  No printf here: a
+// function call inside a kernel that runs wgmma makes ptxas serialise the MMAs.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("odise_b200: mbarrier watchdog block(%d,%d,%d) thread %d\n", blockIdx.x, blockIdx.y, blockIdx.z,
-             threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s at 2 GHz
   }
+}
+// warpgroup-wide register budget (all four warps of the warpgroup execute it): the TMA producer gives registers back,
+// the MMA warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
 }
 
 // ---------------------------------------------------------------- TMA (cp.async.bulk.tensor)
@@ -87,231 +90,42 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// Multicast load: the box lands at the same CTA-relative shared-memory offset in every CTA of `cta_mask` and completes
-// `bytes` on the mbarrier at the same offset in each of them (one L2 read / one crossbar transfer for the whole cluster).
-__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, "
-      "%5}], [%2], %6;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
-      : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
+// named barrier over `threads` threads (a multiple of 32); ids 1.. (0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// all threads of all CTAs of the cluster (release / acquire: barrier inits and shared-memory state become visible)
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// ---- CTA-pair plumbing (cta_group::2 MMAs): address of one of MY shared-memory objects as it appears in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_shared(const void* p, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier of another CTA of the cluster (release at cluster scope)
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a LOCAL mbarrier whose arrivals may come from the peer CTA (acquire at cluster scope); bounded like mbar_wait
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("odise_b200: cluster mbarrier watchdog block(%d,%d,%d) thread %d\n", blockIdx.x, blockIdx.y, blockIdx.z,
-             threadIdx.x);
-      __trap();
-    }
-  }
-}
-
-// TMA store (shared::cta -> global through a tensor map; rows / columns outside the tensor are clipped), bulk-group
-// completion: commit_group closes the stores issued so far by this thread, wait_group.read N blocks until at most N of
-// its groups still have to READ their shared-memory source (the buffer may be overwritten after that).
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// orders this thread's register / shared-memory writes before the wgmma that follow (accumulators, register A fragments)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed groups of this warpgroup still in flight (their accumulators / operands are then free)
 template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// cta_group::2: the TMEM of BOTH CTAs of a pair is allocated / freed together (the same warp id in each CTA executes it)
-__device__ __forceinline__ void tmem_alloc2(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 covers bf16/fp16 inputs with fp32 accumulation.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// The pair forms of the MMAs (issued by one thread of the EVEN CTA of a pair): M = 256 = 128 rows in each CTA's TMEM, the
-// B tile's N rows split half / half over the two CTAs' shared memory (same offsets), each SM reads the peer's half over the
-// SM-to-SM path instead of receiving it from L2.
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma2_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of all prior cta_group::2 MMAs of this thread -> one arrival on the mbarrier at this offset in every CTA of mask
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// all previously issued tcgen05.mma of this thread complete -> one arrival on the mbarrier
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane base + t), columns [c, c+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-// the same arrival delivered to the mbarrier at this offset in every CTA of `cta_mask` (1-SM MMAs fed by multicast TMA: a
-// shared-memory stage may be refilled only when the MMAs of ALL CTAs that received the multicast have read it)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// registers -> TMEM, same shape as tmem_ld16 (thread t of the warp writes row (lane base + t), 16 consecutive fp32 columns)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major operand tile in the canonical SWIZZLE_128B layout: rows of 64 bf16 (128 B), 8-row / 1024 B swizzle
-// atoms stacked along M/N (SBO = 1024 B).  LBO is unused for swizzled K-major (CuTe writes 1).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major operand tile in the canonical SWIZZLE_128B layout: rows of 128 B (64 16-bit or 128 8-bit elements), 8-row /
+// 1024 B swizzle atoms stacked along M/N (SBO = 1024 B); LBO is unused for swizzled K-major (CUTLASS writes 1).  A step of
+// 16 (16-bit) or 32 (8-bit) elements along K inside the atom adds 32 bytes to the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // [0,14)  start address >> 4
   d |= static_cast<uint64_t>(1) << 16;                       // [16,30) LBO >> 4
   d |= static_cast<uint64_t>(1024 >> 4) << 32;               // [32,46) SBO >> 4
-  d |= static_cast<uint64_t>(1) << 46;                       // [46,48) descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                       // [61,64) SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                       // [62,64) SWIZZLE_128B
   return d;
-}
-// bf16 x bf16 -> fp32, M=128, N=n, both operands K-major (InstrDescriptor bit layout, mma_sm100_desc.hpp)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// byte offset of element (row r, 16-byte chunk c) inside a SW128 K-major tile whose rows are 128 B
-__device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t chunk16) {
-  return r * 128u + ((chunk16 ^ (r & 7u)) << 4);
-}
-
-// fp16 x fp16 -> fp32 (a_format bits [7,10) = 0, b_format bits [10,13) = 0).  kind::f16 wants A and B of the SAME 16-bit
-// type: a mixed fp16 x bf16 descriptor raises an illegal-instruction fault on B200 (found on hardware, round 2) — the
-// attention kernel's P (fp16, one plane) therefore multiplies V planes that the projection GEMM emits as fp16 (hi, lo).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 // fp32 -> (hi, lo) bf16 pair with hi + lo ~= x to ~16 mantissa bits (the "bf16x3" operand split)
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
   hi = __float2bfloat16_rn(x);
   lo = __float2bfloat16_rn(x - __bfloat162float(hi));
-}
-
-// D[tmem] (+)= A[smem] * B[smem] on 8-bit float operands (kind::f8f6f4, K = 32 per instruction, fp32 accumulation into the
-// same TMEM accumulator the kind::f16 MMAs of a tile use): twice the MAC rate of the 16-bit kinds.  Operand tiles are the
-// same K-major SWIZZLE_128B layout with 128 one-byte elements per row, so the shared-memory descriptors are those of the
-// 16-bit path byte for byte; the instruction descriptor carries a/b format 1 = E5M2 (the bit pattern of umma_idesc_bf16).
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__host__ __device__ constexpr uint32_t umma_idesc_e5m2(uint32_t m, uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 // the same split into an fp16 pair (11 + 11 mantissa bits; operands of the attention P V product)
@@ -324,14 +138,14 @@ __device__ __forceinline__ void split_f16(float x, uint16_t& hi, uint16_t& lo) {
 
 // ------------------------------------------------------------------------------------------------ operand planes
 // Three formats of the (hi, lo) operand planes of an fp32 matrix [rows, K] (ODISE_PLANES_* in odise_b200.h):
-//   BF16  hi = bf16(x), lo = bf16(x - hi)                         -> bf16x3: hi*hi + hi*lo + lo*hi, 3 MMAs of kind::f16
+//   BF16  hi = bf16(x), lo = bf16(x - hi)                         -> bf16x3: hi*hi + hi*lo + lo*hi, 3 bf16 MMAs
 //   F16   the same with fp16 words (V^T of the attention kernel)
 //   F16Q8 hi = fp16(x);  the second plane has the SAME byte geometry (2 bytes per element, same row stride) but holds,
 //         per block of 64 consecutive k, 64 bytes q_hi[k] = e5m2(x * 2^-S) followed by 64 bytes
 //         q_lo[k] = e5m2((x - hi) * 2^S), S = kQ8Shift.  A GEMM in this format issues, per 64-wide k-block,
-//         4 x kind::f16 (A_hi * B_hi) + 4 x kind::f8f6f4 (A.q_hi * B.q_lo and A.q_lo * B.q_hi, the two first-order
-//         correction terms; the power-of-two scales cancel) = 8 MMA instruction slots instead of the 12 of bf16x3, into one
-//         fp32 TMEM accumulator.  Error per product ~2^-14 (e5m2 keeps 3 significant bits of a term that is itself 2^-12 of
+//         4 x fp16 k16 MMAs (A_hi * B_hi) + 4 x e5m2 k32 MMAs (A.q_hi * B.q_lo and A.q_lo * B.q_hi, the two first-order
+//         correction terms; the power-of-two scales cancel; the 8-bit MMAs run at twice the rate) into one fp32
+//         accumulator.  Error per product ~2^-14 (e5m2 keeps 3 significant bits of a term that is itself 2^-12 of
 //         the product) vs 2^-16 for bf16x3; UNet taps 1.1e-4 vs 2e-5 against the fp32 oracle (tools/precision_budget.py),
 //         bar 1e-3.  Out-of-range values degrade gracefully: a saturated / flushed q byte only perturbs a 2^-12 term.
 // Rows of F16Q8 planes start on 128-byte boundaries (ld % 64 == 0, checked by the host), so the position of an element
@@ -418,6 +232,9 @@ __device__ __forceinline__ void store_planes(__nv_bfloat16* hi, __nv_bfloat16* l
     }
   }
 }
+
+// multiprocessors of the current device (grid sizing of persistent and "one resident wave" launches)
+int num_sms();
 
 // launch-time operand format of the planes written by the producer kernels (odise_set_operand_format)
 int operand_format();

@@ -1,9 +1,9 @@
-"""B200 engine for the Mask2Former half of ODISE (SURVEY.md §8a rows b1-b12): MSDeformAttn pixel decoder
+"""H100 engine for the Mask2Former half of ODISE (SURVEY.md §8a rows b1-b12): MSDeformAttn pixel decoder
 (M2F/modeling/pixel_decoder/msdeformattn.py:314-358), ODISE masked-attention transformer decoder with its pooled
 mask-embedding heads (odise/modeling/meta_arch/odise.py:642-776, :937-1015) and the CLIP-text scoring
 (odise.py:181-207, helper.py:79-109).
 
-Token-major fp32 activations + (hi, lo) bf16 GEMM operands; every contraction is odise_gemm_bf16 (tcgen05), the
+Token-major fp32 activations + (hi, lo) bf16 GEMM operands; every contraction is odise_gemm_bf16 (wgmma), the
 deformable sampling is odise_msda_fused_f32 (softmax + location math + bilinear gathers in one kernel), the masked
 cross-attention never materialises the [B*8, Q, HW] boolean mask (1 bit per (b, q, key), shared by the heads), and
 K / V of the three decoder layers that share a feature level come out of ONE GEMM per level.
@@ -106,7 +106,7 @@ class HeadEngine:
         if self.query_feat.shape[0] != self.Q:
             raise lib.OdiseError(f"num_queries = {self.Q} but query_feat has {self.query_feat.shape[0]} rows")
         for lvl in range(self.n_lvl):   # K / V projections of the layers that read level lvl, concatenated along N and
-            # head-padded 32 -> 64 columns per head (zero rows): the operands of the tcgen05 attention kernel
+            # head-padded 32 -> 64 columns per head (zero rows): the operands of the wgmma attention kernel
             ids = [i for i in range(self.n_dec) if i % self.n_lvl == lvl]
             pad = lambda w: ops.head_pad_rows(w, M_HEADS, D_HEAD, 64)
             padb = lambda b: ops.head_pad_rows(b.view(-1, 1), M_HEADS, D_HEAD, 64).view(-1)

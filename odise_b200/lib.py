@@ -1,6 +1,6 @@
 """ctypes binding of libodise_b200.so (include/odise_b200.h).
 
-PyTorch is used for device memory and streams only; every op here launches hand-written sm_100a kernels through
+PyTorch is used for device memory and streams only; every op here launches hand-written sm_90a kernels through
 the C ABI.  There is NO fallback: if the library is missing or a call fails, an exception is raised.
 """
 import ctypes
@@ -334,9 +334,9 @@ def workspace(nbytes, device):
     return _WS[key]
 
 
-def auto_split(M, N, K, batch=1, sms=148):
+def auto_split(M, N, K, batch=1, sms=132):
     """(force_bn, split_k) for GEMMs that cannot fill the GPU with output tiles alone (e.g. the 8x8 / 16x16 UNet levels:
-    M = 1024 -> 80 tiles of 128 x 128 on 148 SMs).  Cost model in units of K * BN per wave (tools/gemm_one.py), plus
+    M = 1024 -> 80 tiles of 128 x 128 on 132 SMs).  Cost model in units of K * BN per wave (tools/gemm_one.py), plus
     ~6 us for the reduce launch; (0, 1) = leave it to the kernel's own heuristic."""
     tm = (M + 127) // 128
     kblocks = (K + 63) // 64

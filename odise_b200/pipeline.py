@@ -1,4 +1,4 @@
-"""Inference meta-arch of the B200 engine: the eval branch of CategoryODISE.forward
+"""Inference meta-arch of the H100 engine: the eval branch of CategoryODISE.forward
 (odise/modeling/meta_arch/odise.py:209-246, :282-331) restricted to the north-star hot path:
 
     images -> [sliding 512^2 crops] -> UNet feature pass -> projections -> pixel decoder -> masked-attention decoder

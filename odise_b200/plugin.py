@@ -1,4 +1,4 @@
-"""The reference's plugin surface, backed by the B200 engines (SURVEY.md §8b B-1 / B-2 / B-3).
+"""The reference's plugin surface, backed by the H100 engines (SURVEY.md §8b B-1 / B-2 / B-3).
 
 `B200FeatureExtractorBackbone` and `B200MaskFormerHead` keep the forward contracts of
 odise.modeling.backbone.FeatureExtractorBackbone (feature_extractor.py:29-256) and
@@ -21,7 +21,7 @@ ShapeSpec = namedtuple("ShapeSpec", ["channels", "height", "width", "stride"])
 
 def _expect(name, got, want):
     if tuple(got) != tuple(want) if isinstance(want, (tuple, list)) else got != want:
-        raise NotImplementedError(f"{name}={got!r}: the B200 engine implements the released ODISE configuration "
+        raise NotImplementedError(f"{name}={got!r}: the engine implements the released ODISE configuration "
                                   f"({name}={want!r}, configs/common/models/odise_with_label.py)")
 
 
@@ -309,7 +309,7 @@ class B200MaskFormerHead(nn.Module):
             else B200ODISEMultiScaleMaskedTransformerDecoder(num_classes=num_classes)
         for part in (self.pixel_decoder, self.predictor):
             if not isinstance(part, _HeadPart):
-                raise TypeError("pixel_decoder / transformer_predictor must be the B200 plugin classes")
+                raise TypeError("pixel_decoder / transformer_predictor must be the B200* plugin classes")
             object.__setattr__(part, "_owner", self)
         self.in_features = ["s2", "s3", "s4", "s5"] if input_shape is None else \
             [k for k, v in sorted(input_shape.items(), key=lambda kv: kv[1].stride)]

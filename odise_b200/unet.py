@@ -1,9 +1,9 @@
-"""B200 engine for the frozen SD-v1 UNet feature pass of ODISE (SURVEY.md §8a rows a6, a7, a7.1-a7.3).
+"""H100 engine for the frozen SD-v1 UNet feature pass of ODISE (SURVEY.md §8a rows a6, a7, a7.1-a7.3).
 
 Computes exactly what LdmExtractor.unet_forward (odise/modeling/meta_arch/ldm.py:469-491) needs from the UNet at
 t = 0: the inputs of output_blocks[2, 5, 8, 11].  output_blocks[11] and unet.out are never executed (their results
 are discarded by the reference, ldm.py:600).  Layout is NHWC / token-major throughout, so every conv / linear /
-attention projection is one call of the tcgen05 GEMM (odise_gemm_bf16) and the skip concatenations of the up path
+attention projection is one call of the wgmma GEMM (odise_gemm_bf16) and the skip concatenations of the up path
 (torch.cat, ldm.py:485) cost nothing: down-path blocks write their outputs straight into the right half of the
 concat buffer their mirror block will read, up-path blocks into the left half.
 
@@ -142,7 +142,7 @@ class UNetEngine:
     # ------------------------------------------------------------------------------------------- primitives
     def _gemm(self, a, wname, bias=None, **kw):
         if "conv" in kw and kw.get("conv_mode", 0) == 0:
-            # low-resolution levels cannot fill 148 SMs with output tiles: split K (lib.auto_split)
+            # low-resolution levels cannot fill 132 SMs with output tiles: split K (lib.auto_split)
             Mc, Nc, Kc = kw["M"], kw["N"], 9 * kw["conv"][0]
             bn, sk = lib.auto_split(Mc, Nc, Kc)
             if sk > 1:

@@ -1,9 +1,9 @@
-"""B200 engine for the KL-VAE stages of ODISE's feature extractor (SURVEY.md §8f row f-1): the encoder pass that
+"""H100 engine for the KL-VAE stages of ODISE's feature extractor (SURVEY.md §8f row f-1): the encoder pass that
 yields the latent + 2 encoder taps (LdmExtractor.encoder_forward / encode_to_latent, ldm.py:424-467) and the decoder
 pass TRUNCATED after the last tap (decoder_forward, ldm.py:493-533: taps are the inputs of up-blocks 2 and 5; the
 reference runs on to the full 512x512 RGB image and discards it — ~75 % of the decoder FLOPs are dead code).
 
-Same kernels as the UNet ResBlocks: GN(eps 1e-6)+SiLU+split pass -> implicit-GEMM conv3x3 on tcgen05.  The single-head
+Same kernels as the UNet ResBlocks: GN(eps 1e-6)+SiLU+split pass -> implicit-GEMM conv3x3 on wgmma.  The single-head
 4096-token mid-block attention (d = 512) goes through GEMM + odise_softmax_split_f32 + GEMM.
 """
 import torch

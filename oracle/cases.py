@@ -62,4 +62,4 @@ def ldm_case():
     vae = _init(oldm.AutoencoderKL(), 22, 0.03)
     g = torch.Generator().manual_seed(23)
     return dict(unet=unet, vae=vae, x=torch.randn(2, 4, 16, 16, generator=g), ctx=torch.randn(2, 5, 48, generator=g),
-                cond=torch.randn(2, 256, generator=g), img=torch.randn(1, 3, 64, 64, generator=g))
+                cond=torch.randn(2, 256, generator=g), img=torch.randn(1, 3, 32, 32, generator=g))

@@ -1,9 +1,9 @@
 """TEST / BENCH INFRASTRUCTURE (not shipped, not imported by odise_b200/).
 
 ctypes binding of oracle/_ref/libref_msda.so = the REFERENCE's own MSDeformAttn forward CUDA kernel
-(ops/src/cuda/ms_deform_im2col_cuda.cuh:242-304, launcher :928-958) compiled unmodified for sm_100a by oracle/Makefile
+(ops/src/cuda/ms_deform_im2col_cuda.cuh:242-304, launcher :928-958) compiled unmodified for sm_90a by oracle/Makefile
 behind the C shim oracle/ref_msda_host.cu.  Used as (1) a second parity oracle for odise_msda_forward_f32 and (2) the GPU
-baseline the B200 kernel has to beat in the C4 microbench (bench.py --config c4)."""
+baseline the engine's kernel has to beat in the C4 microbench (bench.py --config c4)."""
 import ctypes
 import os
 

@@ -1,7 +1,7 @@
 """Import scaffolding that lets the REFERENCE's own Python (vendored Mask2Former + odise/modeling/meta_arch/odise.py)
 run on CPU in the build container, where detectron2 / fvcore / open_clip / ldm / ... are not installed.
-TEST INFRASTRUCTURE ONLY — used by tools/make_golden_*.py and by CPU tests that are skipped when /root/reference
-is absent (it never exists on the GPU box).  The arithmetic executed is the reference's; only third-party
+TEST INFRASTRUCTURE ONLY — used by tools/make_golden_*.py and by CPU tests, which compute the reference side live
+through it where the reference tree is present and otherwise read what it computed from tests/golden (pinned()).  The arithmetic executed is the reference's; only third-party
 registry / config decorators and the tiny detectron2 layer helpers are stubbed (SURVEY.md Appendix C):
 
   detectron2.layers.Conv2d     = nn.Conv2d with optional .norm / .activation applied in forward  (d2 wrappers.py)
@@ -25,6 +25,47 @@ M2F = os.path.join(REF, "third_party", "Mask2Former")
 
 def available():
     return os.path.isdir(os.path.join(REF, "odise")) and os.path.isdir(os.path.join(M2F, "mask2former"))
+
+
+GOLDEN = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+
+
+def pinned(name, compute, fixture="ref_pinned.pt", store=None):
+    """What the reference's own code yields for `name` (tensors, strings, numbers and containers of them): computed by
+    `compute()` where the reference tree is present, read from tests/golden/<fixture> elsewhere (name None: the whole
+    file is the value).  With ODISE_RECORD_GOLDEN=1 (and the reference present) the computed value, or store(value) when
+    the whole of it would not fit a fixture below 1 MB, is also written to that file; running the CPU tests that way
+    rewrites the fixtures."""
+    path = os.path.join(GOLDEN, fixture)
+    if available():
+        v = compute()
+        if os.environ.get("ODISE_RECORD_GOLDEN") == "1":
+            s = store(v) if store else v
+            if name is None:
+                torch.save(s, path)
+            else:
+                d = torch.load(path, weights_only=True) if os.path.exists(path) else {}
+                d[name] = s
+                torch.save(d, path)
+        return v
+    d = torch.load(path, weights_only=True)
+    return d if name is None else d[name]
+
+
+def sample(t, k=4096, seed=0):
+    """A stored stand-in for a large tensor: `k` seeded flat positions (int32) and the values there."""
+    t = t.detach().reshape(-1)
+    if t.numel() <= k:
+        return dict(idx=torch.arange(t.numel(), dtype=torch.int32), values=t.clone())
+    idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(seed))[:k].sort().values
+    return dict(idx=idx.to(torch.int32), values=t[idx].clone())
+
+
+def at_sample(got, ref):
+    """(got, want): whole tensors when `ref` was computed live, the stored positions of `got` when `ref` is a sample()"""
+    if isinstance(ref, dict):
+        return got.reshape(-1)[ref["idx"].long()], ref["values"]
+    return got, ref
 
 
 class _Anything:

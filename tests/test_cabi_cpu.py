@@ -89,7 +89,7 @@ def test_auto_split_and_struct_layouts():
     import ctypes
     import re
     from odise_b200 import lib
-    # split K only where output tiles alone cannot fill 148 SMs and the partial-sum traffic pays for itself
+    # split K only where output tiles alone cannot fill 132 SMs and the partial-sum traffic pays for itself
     assert lib.auto_split(1024, 1280, 11520) == (160, 2)
     assert lib.auto_split(65536, 320, 2880) == (0, 1) and lib.auto_split(4096, 640, 5760) == (0, 1)
     assert lib.auto_split(256, 1280, 11520)[1] > 1

@@ -18,6 +18,12 @@ def _load(name):
     return torch.load(os.path.join(G, name), map_location="cpu", weights_only=True)
 
 
+def _rounding_level(a, b):
+    """The golden files were written on another CPU, whose kernels may sum in another order: fp32 rounding level,
+    max |a - b| <= 1e-5 max |b| (~1.5e-6 seen between hosts), where the same process would give bit equality."""
+    return a.shape == b.shape and bool((a - b).abs().max() <= 1e-5 * b.abs().max())
+
+
 def _close(a, b, rtol=1e-4, atol=1e-5):
     assert a.shape == b.shape
     assert torch.allclose(a.float(), b, rtol=rtol, atol=atol), (a.float() - b).abs().max().item()
@@ -68,9 +74,10 @@ def test_postprocess_matches_reference_golden():
 def test_ldm_drivers_match_reference_golden():
     ref = _load("ref_ldm_driver.pt")
     d = cases.ldm_case()
-    for a, b in zip(oldm.unet_features(d["unet"], d["x"], d["ctx"], d["cond"]), ref["unet_feats"]):
-        assert torch.equal(a, b)
+    uf = oldm.unet_features(d["unet"], d["x"], d["ctx"], d["cond"])
+    assert len(uf) == len(ref["unet_feats"]) == 4 and all(_rounding_level(a, b) for a, b in zip(uf, ref["unet_feats"]))
     lat, ef = oldm.encoder_features(d["vae"], d["img"])
-    assert torch.equal(lat, ref["latent"]) and all(torch.equal(a, b) for a, b in zip(ef, ref["enc_feats"]))
+    assert _rounding_level(lat, ref["latent"]) and len(ef) == len(ref["enc_feats"])
+    assert all(_rounding_level(a, b) for a, b in zip(ef, ref["enc_feats"]))
     df = oldm.decoder_features(d["vae"], ref["latent"])
-    assert len(df) == 2 and all(torch.equal(a, b) for a, b in zip(df, ref["dec_feats"]))
+    assert len(df) == 2 and all(_rounding_level(a, b) for a, b in zip(df, ref["dec_feats"]))

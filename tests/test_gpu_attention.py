@@ -1,4 +1,4 @@
-"""GPU parity of the fused tcgen05 flash attention (odise_attention_tc) vs fp64 softmax attention.
+"""GPU parity of the fused wgmma flash attention (odise_attention_tc) vs fp64 softmax attention.
 Shapes are the SD-v1 UNet ones: self-attention d=40 / d=80 / d=160, cross-attention over 77 context tokens.
 Tolerance in the bf16x3 mode: the probabilities enter the P V product rounded ONCE to fp16 (2^-12 relative per element,
 random sign -> ~1.5e-4 of the output scale on random data); the budget behind that choice is tools/precision_budget.py
@@ -64,7 +64,7 @@ def test_softmax_split(cuda):
 @pytest.mark.parametrize("nmma", [3, 1])
 @pytest.mark.parametrize("cfg", [(2, 100, 32 * 32, 64, 64), (1, 100, 64 * 64, 256, 256), (2, 37, 8 * 8, 32, 32)])
 def test_masked_attention_tc_d32(cuda, nmma, cfg):
-    """Mask2Former masked cross-attention (odise.py:683-692, 760-774) on the tcgen05 kernel: head dim 32, mask bits from
+    """Mask2Former masked cross-attention (odise.py:683-692, 760-774) on the wgmma kernel: head dim 32, mask bits from
     odise_attn_mask_bits_f32, fully-masked rows attend everywhere."""
     import torch.nn.functional as F
     from odise_b200 import lib, ops

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM / implicit conv (odise_gemm_bf16) against fp64 torch on the same inputs.
+"""GPU parity of the wgmma GEMM / implicit conv (odise_gemm_bf16) against fp64 torch on the same inputs.
 Tolerances: bf16x3 (nmma=3) is the parity mode -> 2e-5 of the output scale; plain bf16 (nmma=1) -> 2e-2."""
 import pytest
 import torch
@@ -256,8 +256,8 @@ def test_groupnorm_statistics_of_a_concat_and_fallbacks(cuda):
     dict(M=256, N=256, K=64, bn=64, batch=3, extra=False),       # batched (decoder-style), one k-block
 ])
 def test_gemm_tma_store_epilogue(cuda, kind, cfg):
-    """One output kind (fp32 OR planes) leaves interior tiles through cp.async.bulk.tensor stores (SASS: UTMASTG): values must
-    equal the fp64 product to the GEMM tolerance, also when the output is a column slice of a wider buffer."""
+    """Single-output GEMMs (fp32 OR planes) on interior and edge tiles: values must equal the fp64 product to the GEMM
+    tolerance, also when the output is a column slice of a wider buffer."""
     from odise_b200 import lib
     M, N, K, Bz = cfg["M"], cfg["N"], cfg["K"], cfg["batch"]
     g = torch.Generator().manual_seed(M + N + K)

@@ -145,7 +145,7 @@ def test_q8_conv3x3_stride2(cuda, mode):
 @pytest.mark.parametrize("kind", ["f32", "planes"])
 @pytest.mark.parametrize("cfg", [(1024, 512, 320, False), (65536, 640, 320, True), (896, 320, 1280, True)])
 def test_q8_tma_store_epilogue(cuda, kind, cfg):
-    """single-output GEMMs leave through TMA stores; F16Q8 planes = fp16 tile + two 16-byte-wide e5m2 boxes per chunk"""
+    """single-output GEMMs in the F16Q8 mode, fp32 or F16Q8 output planes (fp16 tile + the two e5m2 byte blocks per 64 columns)"""
     from odise_b200 import lib
     M, N, K, extra = cfg
     g = torch.Generator().manual_seed(M + N)

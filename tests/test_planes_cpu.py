@@ -70,21 +70,24 @@ def test_producers_refuse_fp16_pairs_and_gemm_checks_formats():
         lib.gemm(a, b, out=torch.empty(128, 128))
 
 
-def test_gemm_tile_policy_follows_the_measured_table():
-    """pick_tile() (csrc/gemm_tc.cu), the cost model behind the GEMM's tile choice, on the shapes its table was measured on
-    (profiles/r2j_gemm_sm2_policy.txt): CTA pairs (2-SM MMAs) only at BN = 256 with K >= 1024 and M tiles that pair up."""
+def test_gemm_tile_policy_cost_model():
+    """pick_tile() (csrc/gemm_tc.cu), the cost model behind the GEMM's tile choice under stream capture: the widest tile
+    that keeps the waves full, 64-wide tiles where fewer output tiles than SMs would be left otherwise, at most 128 columns
+    in the F16Q8 mode (two register accumulators), never CTA pairs."""
     import __graft_entry__ as ge
     ge.build()
     from odise_b200 import lib
-    assert lib.gemm_tile_policy(65536, 512, 4608, conv=True, nmma=2) == (256, True)        # KL-VAE 64x64 conv
-    assert lib.gemm_tile_policy(65536, 512, 4608, conv=True, nmma=3) == (256, True)
-    assert lib.gemm_tile_policy(1048576, 256, 2304, conv=True, nmma=2) == (256, True)      # KL-VAE 256x256 level
-    assert lib.gemm_tile_policy(65536, 320, 2880, conv=True, nmma=2)[1] is False           # UNet 64x64 level: N = 320
-    assert lib.gemm_tile_policy(4194304, 128, 1152, conv=True, nmma=2) == (128, False)     # N = 128: no pair tile
-    assert lib.gemm_tile_policy(9344, 1024, 4096, nmma=2) == (256, True)                    # CLIP MLP projection
-    assert lib.gemm_tile_policy(65536, 640, 320, nmma=2)[1] is False                        # K < 1024: epilogue bound
-    assert lib.gemm_tile_policy(400, 256, 256, nmma=3)[1] is False                          # decoder linears: 4 M tiles
-    assert lib.gemm_tile_policy(100, 256, 256, nmma=3)[1] is False                          # a single M tile cannot pair
-    assert lib.gemm_tile_policy(65536, 512, 4608, nmma=1)[1] is False                       # plain bf16: pairs not instantiated
-    for bn, _ in (lib.gemm_tile_policy(m, n, k, nmma=2) for m in (100, 4096, 65536) for n in (64, 320, 1342) for k in (64, 640, 5760)):
-        assert bn in (64, 128, 160, 256)
+    assert lib.gemm_tile_policy(65536, 512, 4608, conv=True, nmma=3) == (256, False)       # KL-VAE 64x64 conv
+    assert lib.gemm_tile_policy(65536, 512, 4608, conv=True, nmma=2) == (128, False)
+    assert lib.gemm_tile_policy(1048576, 256, 2304, conv=True, nmma=2) == (128, False)     # KL-VAE 256x256 level
+    assert lib.gemm_tile_policy(65536, 320, 2880, conv=True, nmma=2) == (128, False)       # UNet 64x64 level: N = 320
+    assert lib.gemm_tile_policy(4194304, 128, 1152, conv=True, nmma=2) == (128, False)     # N = 128
+    assert lib.gemm_tile_policy(9344, 1024, 4096, nmma=2) == (128, False)                   # CLIP MLP projection
+    assert lib.gemm_tile_policy(65536, 640, 320, nmma=3) == (160, False)                    # K < 1024: epilogue bound
+    assert lib.gemm_tile_policy(400, 256, 256, nmma=3) == (64, False)                       # decoder linears: 4 M tiles
+    assert lib.gemm_tile_policy(100, 256, 256, nmma=3) == (64, False)
+    assert lib.gemm_tile_policy(65536, 512, 4608, nmma=1) == (256, False)
+    for nmma in (1, 2, 3):
+        for bn, pair in (lib.gemm_tile_policy(m, n, k, nmma=nmma) for m in (100, 4096, 65536) for n in (64, 320, 1342)
+                         for k in (64, 640, 5760)):
+            assert bn in ((64, 128) if nmma == 2 else (64, 128, 160, 256)) and pair is False

@@ -1,5 +1,6 @@
 """Vocabulary front end (odise_b200/vocab.py): label files / prompts / overlap rule pinned against the reference's own
-functions and data (skipped without /root/reference), the BPE tokenizer checked on a hand-built merge table."""
+functions and data (what they yield is stored in tests/golden/ref_pinned.pt, oracle.refshim.pinned), the BPE tokenizer
+checked on a hand-built merge table."""
 import os
 
 import pytest
@@ -8,22 +9,37 @@ import torch
 from odise_b200 import vocab
 from oracle import refshim
 
-needs_ref = pytest.mark.skipif(not refshim.available(), reason="/root/reference not present")
-LABELS = "/root/reference/odise/data/datasets/openseg_labels"
+LABELS = os.path.join(refshim.REF, "odise", "data", "datasets", "openseg_labels")
+DATASETS = (("ade20k_150", 150, 403), ("coco_panoptic", 133, 254), ("ade20k_847", 847, 1342))
+PROMPTS = (None, "a", "photo", "scene")
 
 
-@needs_ref
-def test_label_files_and_prompts_match_reference():
+def _label_files(tmp_path, files):
+    """the reference's label files (stored text) written out for vocab.read_label_file"""
+    for name, text in files.items():
+        (tmp_path / name).write_text(text)
+    return str(tmp_path)
+
+
+def test_label_files_and_prompts_match_reference(tmp_path):
     import importlib
-    refshim.install()
-    rb = importlib.import_module("odise.data.build")
-    for name, n_cls, n_prompts in (("ade20k_150", 150, 403), ("coco_panoptic", 133, 254), ("ade20k_847", 847, 1342)):
-        mine = vocab.read_label_file(os.path.join(LABELS, f"{name}_with_prompt_eng.txt"))
-        ref = rb.get_openseg_labels(name, prompt_engineered=True)
-        assert mine == ref and len(mine) == n_cls and sum(len(s) for s in mine) == n_prompts     # SURVEY.md §8 K' counts
-        for p in (None, "a", "photo", "scene"):
-            assert vocab.prompt_labels(mine, p) == rb.prompt_labels(ref, p)
-    assert vocab.read_label_file(os.path.join(LABELS, "ade20k_150.txt")) == rb.get_openseg_labels("ade20k_150")
+
+    def ref():
+        refshim.install()
+        rb = importlib.import_module("odise.data.build")
+        names = [f"{n}_with_prompt_eng.txt" for n, _, _ in DATASETS] + ["ade20k_150.txt"]
+        labels = {n: rb.get_openseg_labels(n, prompt_engineered=True) for n, _, _ in DATASETS}
+        return dict(files={f: open(os.path.join(LABELS, f)).read() for f in names}, labels=labels,
+                    plain=rb.get_openseg_labels("ade20k_150"),
+                    prompts={f"{n}/{p}": rb.prompt_labels(labels[n], p) for n, _, _ in DATASETS for p in PROMPTS})
+    r = refshim.pinned("openseg_labels", ref)
+    d = _label_files(tmp_path, r["files"])
+    for name, n_cls, n_prompts in DATASETS:
+        mine = vocab.read_label_file(os.path.join(d, f"{name}_with_prompt_eng.txt"))
+        assert mine == r["labels"][name] and len(mine) == n_cls and sum(len(s) for s in mine) == n_prompts   # SURVEY.md §8 K'
+        for p in PROMPTS:
+            assert vocab.prompt_labels(mine, p) == r["prompts"][f"{name}/{p}"]
+    assert vocab.read_label_file(os.path.join(d, "ade20k_150.txt")) == r["plain"]
 
 
 def test_overlap_rule():
@@ -128,21 +144,35 @@ def test_open_state_dict_protocol_swaps_vocabularies():
         bare.load_open_state_dict({"category_head.test_labels": la, "clip_head.test_labels": la})
 
 
-@needs_ref
-def test_prompts_of_the_two_heads_match_reference():
+def _prompt_facts(cfg):
+    """what the label config says about the two heads' prompts (only these facts are kept, not the file)"""
+    return dict(category_head_sets_prompt="prompt=" in cfg.split("category_head=")[1].split("clip_head=")[0],
+                clip_head_default="clip_head=L(PoolingCLIPHead)()" in cfg)
+
+
+def test_prompts_of_the_two_heads_match_reference(tmp_path):
     """ADVICE r1 (high): in the label model the category head scores against the RAW class names (CategoryEmbed
     prompt=None, odise.py:1225; configs/common/models/mask_generator_with_label.py passes none) and only PoolingCLIPHead
     uses "a photo of a {}." (odise.py:1428).  Pinned on the reference's own defaults and prompt function."""
     import inspect
-    od = refshim.modules().odise_module
-    assert inspect.signature(od.CategoryEmbed.__init__).parameters["prompt"].default is None
-    assert inspect.signature(od.PoolingCLIPHead.__init__).parameters["prompt"].default == "photo"
-    cfg = open("/root/reference/configs/common/models/mask_generator_with_label.py").read()
-    assert "prompt=" not in cfg.split("category_head=")[1].split("clip_head=")[0]
-    assert "clip_head=L(PoolingCLIPHead)()" in cfg
-    labels = vocab.read_label_file(os.path.join(LABELS, "ade20k_150_with_prompt_eng.txt"))
+
+    def ref():
+        od = refshim.modules().odise_module
+        cat_p = inspect.signature(od.CategoryEmbed.__init__).parameters["prompt"].default
+        clip_p = inspect.signature(od.PoolingCLIPHead.__init__).parameters["prompt"].default
+        name = "ade20k_150_with_prompt_eng.txt"
+        text = open(os.path.join(LABELS, name)).read()
+        labels = vocab.read_label_file(os.path.join(LABELS, name))
+        return dict(cat_prompt=cat_p, clip_prompt=clip_p, files={name: text},
+                    **_prompt_facts(open(os.path.join(refshim.REF, "configs/common/models/mask_generator_with_label.py")).read()),
+                    want_cat=od.prompt_labels(labels, cat_p), want_clip=od.prompt_labels(labels, clip_p))
+    r = refshim.pinned("head_prompts", ref)
+    assert r["cat_prompt"] is None
+    assert r["clip_prompt"] == "photo"
+    assert not r["category_head_sets_prompt"]
+    assert r["clip_head_default"]
+    labels = vocab.read_label_file(os.path.join(_label_files(tmp_path, r["files"]), "ade20k_150_with_prompt_eng.txt"))
     cat, clip, sizes = vocab.vocabulary_prompts(labels)
-    want_cat = od.prompt_labels(labels, inspect.signature(od.CategoryEmbed.__init__).parameters["prompt"].default)
-    want_clip = od.prompt_labels(labels, inspect.signature(od.PoolingCLIPHead.__init__).parameters["prompt"].default)
+    want_cat, want_clip = r["want_cat"], r["want_clip"]
     assert cat == [p for s_ in want_cat for p in s_] and clip == [p for s_ in want_clip for p in s_]
     assert sizes == [len(s_) for s_ in labels] and len(cat) == len(clip) == 403 and cat != clip

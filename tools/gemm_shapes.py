@@ -29,11 +29,11 @@ n, ms, fl = lib.profile_end()
 print(f"{n} gemm launches, {ms:.2f} ms, {fl/ms/1e9:.1f} TFLOP/s algorithmic")
 agg = defaultdict(lambda: [0, 0.0, 0.0])
 for line in open(out).read().splitlines()[1:]:
-    M, N, K, b, conv, bn, nm, sp, t, tf, pair = line.split(",")
-    k = (int(M), int(N), int(K), int(b), int(conv), int(bn), int(sp), int(nm), int(pair))
+    M, N, K, b, conv, bn, nm, sp, t, tf = line.split(",")
+    k = (int(M), int(N), int(K), int(b), int(conv), int(bn), int(sp), int(nm))
     agg[k][0] += 1
     agg[k][1] += float(t)
     agg[k][2] += 2.0 * int(M) * int(N) * int(K) * int(b)
-print("   ms    n   TF/s  (M, N, K, batch, conv, BN, splits, nmma, pair: 0 single / 1 multicast / 2 = 2-SM MMAs)")
+print("   ms    n   TF/s  (M, N, K, batch, conv, BN, splits, nmma)")
 for k, (c, t, f) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:45]:
     print(f"{t:7.3f} {c:4d} {f/t/1e9:6.0f}  {k}")

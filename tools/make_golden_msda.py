@@ -37,5 +37,5 @@ def make(name, seed, N, M, D, shapes, Lq, P, spread=1.0):
 
 if __name__ == "__main__":
     make("reftest", 3, 1, 2, 2, [(6, 4), (3, 2)], 2, 2)                       # exact ops/test.py problem
-    make("d32_small", 11, 2, 8, 32, [(4, 4), (8, 8), (16, 16)], 150, 4, spread=1.3)
+    make("d32_small", 11, 2, 8, 32, [(4, 4), (8, 8), (12, 12)], 100, 4, spread=1.3)
     make("oob", 12, 1, 4, 8, [(5, 7), (3, 2)], 41, 3, spread=3.0)

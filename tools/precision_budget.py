@@ -1,6 +1,6 @@
 """Error budget of cheaper tensor-core precision modes for the UNet feature pass (VERDICT r1 item 4a), by EMULATION on the
 CPU oracle: every contraction of the SD-v1 UNet (3x3 convs | 1x1 convs + linears | attention QK^T and PV) is run with its
-operands rounded the way a given tcgen05 scheme would see them, and the four taps are compared with the plain fp32 oracle
+operands rounded the way a given tensor-core scheme would see them, and the four taps are compared with the plain fp32 oracle
 (the parity reference; bar 1e-3 on max|a-b| / max|b|, ship rule: >= 3x margin -> <= 3.3e-4).
 
 Schemes (cost in bf16-MMA units per k-step; bf16x3 = what the engine ships):
@@ -10,7 +10,7 @@ Schemes (cost in bf16-MMA units per k-step; bf16x3 = what the engine ships):
   bf16x2     same with bf16 planes                                      cost 2
   tf32       kind::tf32, both operands rounded to 10 mantissa bits (RN; the hardware truncates: tf32t)   cost 2
   bf16       plain bf16                                                 cost 1
-Usage: python tools/precision_budget.py [--latent 64] > profiles/r2_precision_budget.txt"""
+Usage: python tools/precision_budget.py [--latent 64]"""
 import argparse
 import os
 import sys
@@ -147,8 +147,8 @@ def main():
 
     cost = {"fp32": None, "bf16x3": 3, "fp16x3": 3, "fp16x2": 2, "bf16x2": 2, "tf32": 2, "tf32t": 2, "bf16": 1, "fp16x2c8": 2.5,
             "p16": 2.5, "f16c8": 2, "f16c8e4": 2}
-    # MMA-FLOP share of the three classes in the minimal feature pass (profiles/r1*_gemm_shapes: convs ~ 62 %, linears /
-    # 1x1 ~ 30 %, attention ~ 8 %) -> relative tensor time of a mix vs all-bf16x3
+    # MMA-FLOP share of the three classes in the minimal feature pass (per-GEMM shapes of one step, tools/gemm_shapes.py:
+    # convs ~ 62 %, linears / 1x1 ~ 30 %, attention ~ 8 %) -> relative tensor time of a mix vs all-bf16x3
     share = {"conv3": 0.62, "lin": 0.30, "attn": 0.08}
     print(f"# UNet taps (blocks 2, 5, 8, 11) at a {L}x{L} latent, synthetic weights seed 0; rel = max|a-b| / max|b| vs the fp32 oracle")
     print(f"# {'conv3x3':8s} {'linear':8s} {'attn':8s} | {'tap2':>9s} {'tap5':>9s} {'tap8':>9s} {'tap11':>9s} | {'worst':>9s} | tensor time vs bf16x3 | ships (<= 3.3e-4)")

@@ -1,8 +1,9 @@
 #!/usr/bin/env bash
 # compute-sanitizer over the smoke path (SURVEY.md §5 "race detection"): memcheck finds out-of-bounds / misaligned accesses
-# of the hand-written kernels, racecheck shared-memory hazards, synccheck barrier misuse.  Run on a GPU box:
-#     gpurun --timeout 1500 -- 'bash tools/sanitize.sh memcheck > gpurun_out/sanitize_memcheck.log 2>&1'
-# The TMA / tcgen05 kernels are covered by memcheck (global side) only: racecheck does not model the async proxy.
+# of the hand-written kernels, racecheck shared-memory hazards, synccheck barrier misuse.  On a machine with a GPU and
+# compute-sanitizer:
+#     bash tools/sanitize.sh memcheck > sanitize_memcheck.log 2>&1
+# The TMA / wgmma kernels are covered by memcheck (global side) only: racecheck does not model the async proxy.
 set -u
 TOOL=${1:-memcheck}
 cd "$(dirname "$0")/.."
