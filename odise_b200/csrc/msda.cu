@@ -8,6 +8,8 @@
 // own one (query, head) pair, each lane gathers 16-byte channel vectors, so a D=32 head is 8 lanes x float4 and a
 // warp keeps 4 pairs x 48 independent 128-bit gathers in flight.  HBM/L2-bound: value (22 MB/image) stays
 // L2-resident, loc/attn/out stream once.
+#include <type_traits>
+
 #include "ptx.cuh"
 #include "odise_b200.h"
 #include "launch_count.h"
@@ -108,10 +110,11 @@ msda_vec4_kernel(const float* __restrict__ value, const MsdaLevels lv, const flo
   }
 }
 
-// generic scalar path (any D, e.g. the D=2 problem of the reference's ops/test.py:24-31)
-__global__ void msda_scalar_kernel(const float* __restrict__ value, const MsdaLevels lv,
-                                   const float* __restrict__ loc, const float* __restrict__ attn,
-                                   float* __restrict__ out, int N, int S, int M, int D, int L, int Lq, int P) {
+// generic scalar path (any D, e.g. the D=2 problem of the reference's ops/test.py:24-31); T = float or double
+template <typename T>
+__global__ void msda_scalar_kernel(const T* __restrict__ value, const MsdaLevels lv,
+                                   const T* __restrict__ loc, const T* __restrict__ attn,
+                                   T* __restrict__ out, int N, int S, int M, int D, int L, int Lq, int P) {
   const long long total = (long long)N * Lq * M * D;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -120,19 +123,19 @@ __global__ void msda_scalar_kernel(const float* __restrict__ value, const MsdaLe
     const int m = (int)(pair % M);
     const int n = (int)(pair / M / Lq);
     const int pix_stride = M * D;
-    const float* vb = value + (long long)n * S * pix_stride + m * D + c;
-    float col = 0.f;
+    const T* vb = value + (long long)n * S * pix_stride + m * D + c;
+    T col = 0;
     for (int l = 0; l < L; ++l) {
       const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
-      const float* vl = vb + (long long)__ldg(lv.start + l) * pix_stride;
+      const T* vl = vb + (long long)__ldg(lv.start + l) * pix_stride;
       for (int p = 0; p < P; ++p) {
-        const float lx = loc[(pair * L * P + l * P + p) * 2], ly = loc[(pair * L * P + l * P + p) * 2 + 1];
-        const float aw = attn[pair * L * P + l * P + p];
-        const float h_im = ly * H - 0.5f, w_im = lx * W - 0.5f;
-        if (h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W) {
-          const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-          const float lh = h_im - h_low, lw = w_im - w_low, hh = 1.f - lh, hw = 1.f - lw;
-          float v1 = 0, v2 = 0, v3 = 0, v4 = 0;
+        const T lx = loc[(pair * L * P + l * P + p) * 2], ly = loc[(pair * L * P + l * P + p) * 2 + 1];
+        const T aw = attn[pair * L * P + l * P + p];
+        const T h_im = ly * H - (T)0.5, w_im = lx * W - (T)0.5;
+        if (h_im > (T)-1 && w_im > (T)-1 && h_im < (T)H && w_im < (T)W) {
+          const int h_low = (int)floor(h_im), w_low = (int)floor(w_im);
+          const T lh = h_im - h_low, lw = w_im - w_low, hh = (T)1 - lh, hw = (T)1 - lw;
+          T v1 = 0, v2 = 0, v3 = 0, v4 = 0;
           if (h_low >= 0 && w_low >= 0) v1 = vl[(long long)(h_low * W + w_low) * pix_stride];
           if (h_low >= 0 && w_low + 1 <= W - 1) v2 = vl[(long long)(h_low * W + w_low + 1) * pix_stride];
           if (h_low + 1 <= H - 1 && w_low >= 0) v3 = vl[(long long)((h_low + 1) * W + w_low) * pix_stride];
@@ -157,6 +160,37 @@ __global__ void msda_scalar_kernel(const float* __restrict__ value, const MsdaLe
 // (ncu r1: 396 M warp instructions, issue-bound); what remains is the L1/L2 data path: 4 corners x 128 B per
 // (query, head, sample) = 48 x 128 B lines per pair.
 constexpr int MSDA_PAIRS = 32;
+
+// The bilinear footprint of one sample, shared by the D = 32 forward and backward kernels: the four corners
+// (top-left, top-right, bottom-left, bottom-right) as 32-bit element offsets from the (image, head) base with the level
+// start folded in, their bilinear weights, the fractional position (lh, lw) and a bit per corner that lies inside the
+// level.  Corners outside the level (and every corner of a sample outside it) get offset 0, weight 0 and no bit.
+struct MsdaCorners {
+  int4 off;
+  float4 w;
+  float lh, lw;
+  int valid;
+};
+
+__device__ __forceinline__ MsdaCorners msda_corners(float lx, float ly, int H, int W, int start, int pix) {
+  MsdaCorners c;
+  c.off = make_int4(0, 0, 0, 0);
+  c.w = make_float4(0.f, 0.f, 0.f, 0.f);
+  c.lh = 0.f; c.lw = 0.f; c.valid = 0;
+  const float h_im = ly * H - 0.5f, w_im = lx * W - 0.5f;
+  if (h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W) {
+    const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
+    const float lh = h_im - h_low, lw = w_im - w_low, hh = 1.f - lh, hw = 1.f - lw;
+    const bool t = h_low >= 0, b = h_low + 1 <= H - 1, lf = w_low >= 0, rt = w_low + 1 <= W - 1;
+    const int base = (start + h_low * W + w_low) * pix;
+    c.lh = lh; c.lw = lw;
+    if (t && lf) { c.off.x = base; c.w.x = hh * hw; c.valid |= 1; }
+    if (t && rt) { c.off.y = base + pix; c.w.y = hh * lw; c.valid |= 2; }
+    if (b && lf) { c.off.z = base + W * pix; c.w.z = lh * hw; c.valid |= 4; }
+    if (b && rt) { c.off.w = base + (W + 1) * pix; c.w.w = lh * lw; c.valid |= 8; }
+  }
+  return c;
+}
 
 template <int FUSED>
 __global__ void __launch_bounds__(256)
@@ -203,21 +237,9 @@ msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const floa
       aw = e / sum;
     }
     if (live) {
-      const float h_im = ly * H - 0.5f, w_im = lx * W - 0.5f;
-      int4 o4 = make_int4(0, 0, 0, 0);
-      float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W) {
-        const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-        const float lh = h_im - h_low, lw = w_im - w_low, hh = 1.f - lh, hw = 1.f - lw;
-        const bool t = h_low >= 0, b = h_low + 1 <= H - 1, lf = w_low >= 0, rt = w_low + 1 <= W - 1;
-        const int base = (start + h_low * W + w_low) * pix;
-        if (t && lf) { o4.x = base; w4.x = hh * hw * aw; }
-        if (t && rt) { o4.y = base + pix; w4.y = hh * lw * aw; }
-        if (b && lf) { o4.z = base + W * pix; w4.z = lh * hw * aw; }
-        if (b && rt) { o4.w = base + (W + 1) * pix; w4.w = lh * lw * aw; }
-      }
-      s_off[pl * LP + s] = o4;
-      s_w[pl * LP + s] = w4;
+      const MsdaCorners cn = msda_corners(lx, ly, H, W, start, pix);
+      s_off[pl * LP + s] = cn.off;
+      s_w[pl * LP + s] = make_float4(cn.w.x * aw, cn.w.y * aw, cn.w.z * aw, cn.w.w * aw);
     }
   }
   __syncthreads();
@@ -268,6 +290,182 @@ static void launch_d32(const float* value, const MsdaLevels& lv, const float* a,
 
 static bool vec_ok(int D) { return D % 4 == 0 && D <= 128 && (32 % (D / 4) == 0); }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Backward: ms_deformable_col2im_gpu_kernel / ms_deform_attn_col2im_bilinear of the reference (.cuh:92-164, launcher
+// ms_deform_attn_cuda.cu:88-158).  For every sample inside its level (-1 < h < H, -1 < w < W) and every corner inside
+// the level:
+//   grad_value[corner] += w_corner * attn * g,      grad_attn = sum_c g_c * bilinear_c,
+//   grad_loc.x = W * attn * sum_c g_c * d bilinear_c / dw,   grad_loc.y = H * attn * sum_c g_c * d bilinear_c / dh.
+// Corners outside the level contribute nothing to any of the three (the reference's per-corner `if`: their value is
+// never read); samples outside the level get grad_loc = grad_attn = 0.
+
+__device__ __forceinline__ float4 scale4(const float4& v, float s) {
+  return make_float4(v.x * s, v.y * s, v.z * s, v.w * s);
+}
+__device__ __forceinline__ float dot4(const float4& a, const float4& b) {
+  return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+}
+
+// D = 32: the forward's block of MSDA_PAIRS pairs.  Phase 1 stores per (pair, sample) the corners of msda_corners with
+// their bits and the attention weight; phase 2 runs 8 lanes per pair with one float4 of channels each (grad_out loaded
+// once per pair).  Per sample a lane does four LDG.128 of value, three partial dot products (bilinear value, d/dh,
+// d/dw) and up to four 128-bit vector reductions into grad_value (atomicAdd(float4*) -> REDG.E.ADD.F32x4, a quarter of
+// the reference's scalar atomics).  The partials are summed over the 8 lanes with xor shuffles and one lane stores
+// grad_attn and grad_loc: no atomics there, so both are bit-deterministic; only grad_value depends on the order of the
+// reductions, as in the reference.
+__global__ void __launch_bounds__(256)
+msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, const float* __restrict__ loc,
+                         const float* __restrict__ attn, const float* __restrict__ grad_out,
+                         float* __restrict__ grad_value, float* __restrict__ grad_loc, float* __restrict__ grad_attn,
+                         int N, int S, int M, int L, int Lq, int P) {
+  extern __shared__ __align__(16) uint8_t msda_smem[];
+  const int LP = L * P;
+  int4* s_off = reinterpret_cast<int4*>(msda_smem);                                   // [PAIRS][LP]
+  float4* s_w = reinterpret_cast<float4*>(msda_smem + (size_t)MSDA_PAIRS * LP * sizeof(int4));
+  float4* s_f = s_w + MSDA_PAIRS * LP;                                                // (lh, lw, attn, corner bits)
+  const long long pairs = (long long)N * Lq * M;
+  const long long pair0 = (long long)blockIdx.x * MSDA_PAIRS;
+  const int pix = M * 32;
+
+  // ---- phase 1: (pair, sample) slots; pairs past the end get zero corners so that their lanes do no memory work
+  for (int slot = threadIdx.x; slot < MSDA_PAIRS * LP; slot += 256) {
+    const int pl = slot / LP, s = slot - pl * LP;
+    const long long pair = pair0 + pl;
+    int4 o4 = make_int4(0, 0, 0, 0);
+    float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
+    if (pair < pairs) {
+      const int l = s / P;
+      const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
+      const int start = (int)__ldg(lv.start + l);
+      const float2 xy = __ldg(reinterpret_cast<const float2*>(loc + (pair * LP + s) * 2));
+      const MsdaCorners cn = msda_corners(xy.x, xy.y, H, W, start, pix);
+      o4 = cn.off;
+      w4 = cn.w;
+      f4 = make_float4(cn.lh, cn.lw, __ldg(attn + pair * LP + s), __int_as_float(cn.valid));
+    }
+    s_off[slot] = o4;
+    s_w[slot] = w4;
+    s_f[slot] = f4;
+  }
+  __syncthreads();
+
+  // ---- phase 2: 8 lanes per pair, float4 of channels per lane; every lane runs every sample (the shuffles need them)
+  const int pl = threadIdx.x >> 3;
+  const long long pair = pair0 + pl;
+  const bool live = pair < pairs;
+  const int c = (threadIdx.x & 7) * 4;
+  const int m = (int)(pair % M);
+  const int n = (int)(pair / M / Lq);
+  const long long vbase = (long long)n * S * pix + m * 32 + c;
+  const float* vb = value + vbase;
+  float* gvb = grad_value + vbase;
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 g = live ? ld4(grad_out + pair * 32 + c) : zero;
+  const int4* po = s_off + pl * LP;
+  const float4* pw = s_w + pl * LP;
+  const float4* pf = s_f + pl * LP;
+  for (int l = 0, s = 0; l < L; ++l) {
+    const float Hf = (float)__ldg(lv.shapes + 2 * l), Wf = (float)__ldg(lv.shapes + 2 * l + 1);
+#pragma unroll 2
+    for (int p = 0; p < P; ++p, ++s) {
+      const int4 o4 = po[s];
+      const float4 w4 = pw[s], f4 = pf[s];
+      const int valid = __float_as_int(f4.w);
+      const float4 v1 = (valid & 1) ? ld4(vb + o4.x) : zero, v2 = (valid & 2) ? ld4(vb + o4.y) : zero,
+                   v3 = (valid & 4) ? ld4(vb + o4.z) : zero, v4 = (valid & 8) ? ld4(vb + o4.w) : zero;
+      const float lh = f4.x, lw = f4.y, hh = 1.f - lh, hw = 1.f - lw, aw = f4.z;
+      float4 bil, dh, dw;
+      bil.x = w4.x * v1.x + w4.y * v2.x + w4.z * v3.x + w4.w * v4.x;
+      bil.y = w4.x * v1.y + w4.y * v2.y + w4.z * v3.y + w4.w * v4.y;
+      bil.z = w4.x * v1.z + w4.y * v2.z + w4.z * v3.z + w4.w * v4.z;
+      bil.w = w4.x * v1.w + w4.y * v2.w + w4.z * v3.w + w4.w * v4.w;
+      dh.x = hw * (v3.x - v1.x) + lw * (v4.x - v2.x);
+      dh.y = hw * (v3.y - v1.y) + lw * (v4.y - v2.y);
+      dh.z = hw * (v3.z - v1.z) + lw * (v4.z - v2.z);
+      dh.w = hw * (v3.w - v1.w) + lw * (v4.w - v2.w);
+      dw.x = hh * (v2.x - v1.x) + lh * (v4.x - v3.x);
+      dw.y = hh * (v2.y - v1.y) + lh * (v4.y - v3.y);
+      dw.z = hh * (v2.z - v1.z) + lh * (v4.z - v3.z);
+      dw.w = hh * (v2.w - v1.w) + lh * (v4.w - v3.w);
+      float sv = dot4(g, bil), sh = dot4(g, dh), sw = dot4(g, dw);
+      if (valid & 1) atomicAdd(reinterpret_cast<float4*>(gvb + o4.x), scale4(g, w4.x * aw));
+      if (valid & 2) atomicAdd(reinterpret_cast<float4*>(gvb + o4.y), scale4(g, w4.y * aw));
+      if (valid & 4) atomicAdd(reinterpret_cast<float4*>(gvb + o4.z), scale4(g, w4.z * aw));
+      if (valid & 8) atomicAdd(reinterpret_cast<float4*>(gvb + o4.w), scale4(g, w4.w * aw));
+      for (int o = 4; o; o >>= 1) {
+        sv += __shfl_xor_sync(0xffffffffu, sv, o);
+        sh += __shfl_xor_sync(0xffffffffu, sh, o);
+        sw += __shfl_xor_sync(0xffffffffu, sw, o);
+      }
+      if (live && c == 0) {
+        const long long i = pair * LP + s;
+        grad_attn[i] = sv;
+        *reinterpret_cast<float2*>(grad_loc + 2 * i) = make_float2(Wf * aw * sw, Hf * aw * sh);
+      }
+    }
+  }
+}
+
+// Generic path (any D, float or double, 64-bit offsets): one warp per (query, head) pair, lanes stride over the
+// channels, the three partials are summed with warp shuffles and lane 0 stores grad_attn / grad_loc.  grad_value takes
+// plain scalar atomics (native for double on sm_90).
+template <typename T>
+__global__ void __launch_bounds__(256)
+msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc,
+                          const T* __restrict__ attn, const T* __restrict__ grad_out, T* __restrict__ grad_value,
+                          T* __restrict__ grad_loc, T* __restrict__ grad_attn, int N, int S, int M, int D, int L,
+                          int Lq, int P) {
+  const long long pair = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  if (pair >= (long long)N * Lq * M) return;        // whole warps leave together
+  const int lane = threadIdx.x & 31;
+  const int m = (int)(pair % M);
+  const long long n = pair / M / Lq;
+  const long long pix = (long long)M * D;
+  const long long vbase = n * S * pix + (long long)m * D;
+  const T* vb = value + vbase;
+  T* gvb = grad_value + vbase;
+  const T* go = grad_out + pair * D;
+  for (int l = 0; l < L; ++l) {
+    const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
+    const long long start = __ldg(lv.start + l);
+    for (int p = 0; p < P; ++p) {
+      const long long i = (pair * L + l) * P + p;
+      const T lx = loc[2 * i], ly = loc[2 * i + 1], aw = attn[i];
+      const T h_im = ly * H - (T)0.5, w_im = lx * W - (T)0.5;
+      T sv = 0, sh = 0, sw = 0;
+      if (h_im > (T)-1 && w_im > (T)-1 && h_im < (T)H && w_im < (T)W) {
+        const int h_low = (int)floor(h_im), w_low = (int)floor(w_im);
+        const T lh = h_im - h_low, lw = w_im - w_low, hh = (T)1 - lh, hw = (T)1 - lw;
+        const T w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
+        const bool t = h_low >= 0, b = h_low + 1 <= H - 1, lf = w_low >= 0, rt = w_low + 1 <= W - 1;
+        const long long o1 = (start + (long long)h_low * W + w_low) * pix, o2 = o1 + pix, o3 = o1 + W * pix,
+                        o4 = o3 + pix;
+        for (int c = lane; c < D; c += 32) {
+          const T gc = go[c], ga = gc * aw;
+          T v1 = 0, v2 = 0, v3 = 0, v4 = 0;
+          if (t && lf) { v1 = vb[o1 + c]; atomicAdd(gvb + o1 + c, w1 * ga); }
+          if (t && rt) { v2 = vb[o2 + c]; atomicAdd(gvb + o2 + c, w2 * ga); }
+          if (b && lf) { v3 = vb[o3 + c]; atomicAdd(gvb + o3 + c, w3 * ga); }
+          if (b && rt) { v4 = vb[o4 + c]; atomicAdd(gvb + o4 + c, w4 * ga); }
+          sv += gc * (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4);
+          sh += gc * (hw * (v3 - v1) + lw * (v4 - v2));
+          sw += gc * (hh * (v2 - v1) + lh * (v4 - v3));
+        }
+      }
+      for (int o = 16; o; o >>= 1) {
+        sv += __shfl_xor_sync(0xffffffffu, sv, o);
+        sh += __shfl_xor_sync(0xffffffffu, sh, o);
+        sw += __shfl_xor_sync(0xffffffffu, sw, o);
+      }
+      if (lane == 0) {
+        grad_attn[i] = sv;
+        grad_loc[2 * i] = (T)W * aw * sw;
+        grad_loc[2 * i + 1] = (T)H * aw * sh;
+      }
+    }
+  }
+}
+
 }  // namespace ob
 
 using namespace ob;
@@ -291,10 +489,75 @@ extern "C" int odise_msda_forward_f32(const float* value, const int64_t* spatial
     const long long total = (long long)N * Lq * M * D;
     int blocks = (int)((total + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-    msda_scalar_kernel<<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
+    msda_scalar_kernel<float><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
   }
   count_launch(1);
   return (int)cudaGetLastError();
+}
+
+extern "C" int odise_msda_forward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const double* loc, const double* attn, double* out, int N, int S, int M, int D,
+                                      int L, int Lq, int P, void* stream_v) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  if (!value || !spatial_shapes || !level_start || !loc || !attn || !out) return ODISE_ERR_ARG;
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  MsdaLevels lv{spatial_shapes, level_start};
+  const long long total = (long long)N * Lq * M * D;
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+  msda_scalar_kernel<double><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
+  count_launch(1);
+  return (int)cudaGetLastError();
+}
+
+template <typename T>
+static int msda_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start, const T* loc,
+                         const T* attn, const T* grad_out, T* grad_value, T* grad_loc, T* grad_attn, int N, int S, int M,
+                         int D, int L, int Lq, int P, void* stream_v) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  if (!value || !spatial_shapes || !level_start || !loc || !attn || !grad_out || !grad_value || !grad_loc || !grad_attn)
+    return ODISE_ERR_ARG;
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  const long long pairs = (long long)N * Lq * M;
+  if ((pairs + 7) / 8 > 0x7fffffffLL) return ODISE_ERR_ARG;   // grid of the generic path
+  MsdaLevels lv{spatial_shapes, level_start};
+  // the reference returns at::zeros_like(value) plus the scattered contributions
+  cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(T) * (size_t)N * S * M * D, stream);
+  if (e != cudaSuccess) return (int)e;
+  bool d32 = false;
+  if constexpr (std::is_same<T, float>::value) {
+    if (d32_ok(S, M, D, L, P)) {
+      // 48 B of shared memory per (pair, sample): at most 32 x 32 x 48 = 48 KB, the default dynamic limit
+      const size_t smem = (size_t)MSDA_PAIRS * L * P * (sizeof(int4) + 2 * sizeof(float4));
+      const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
+      msda_d32_backward_kernel<<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value, grad_loc,
+                                                              grad_attn, N, S, M, L, Lq, P);
+      d32 = true;
+    }
+  }
+  if (!d32) {
+    const long long blocks = (pairs + 7) / 8;       // one warp per (query, head) pair
+    msda_backward_warp_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(value, lv, loc, attn, grad_out, grad_value,
+                                                                       grad_loc, grad_attn, N, S, M, D, L, Lq, P);
+  }
+  count_launch(1);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int odise_msda_backward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                       const float* loc, const float* attn, const float* grad_out, float* grad_value,
+                                       float* grad_loc, float* grad_attn, int N, int S, int M, int D, int L, int Lq,
+                                       int P, void* stream) {
+  return msda_backward<float>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,
+                              N, S, M, D, L, Lq, P, stream);
+}
+
+extern "C" int odise_msda_backward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                       const double* loc, const double* attn, const double* grad_out,
+                                       double* grad_value, double* grad_loc, double* grad_attn, int N, int S, int M,
+                                       int D, int L, int Lq, int P, void* stream) {
+  return msda_backward<double>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc,
+                               grad_attn, N, S, M, D, L, Lq, P, stream);
 }
 
 extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,

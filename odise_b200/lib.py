@@ -49,6 +49,9 @@ _lib = None
 _SIGS = {
     "odise_msda_forward_f32": [c_void_p] * 6 + [c_int] * 7 + [c_void_p],
     "odise_msda_fused_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
+    "odise_msda_forward_f64": [c_void_p] * 6 + [c_int] * 7 + [c_void_p],
+    "odise_msda_backward_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
+    "odise_msda_backward_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -461,6 +464,63 @@ def msda_forward(value, spatial_shapes, level_start_index, sampling_locations, a
                                          _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P, _stream()),
            "odise_msda_forward_f32")
     return out
+
+
+def _msda_inputs(tensors, im2col_step):
+    """Checks of ms_deform_attn_cuda_forward / _backward (reference .cu:33-57, :98-121) for the float / double entry
+    points: CUDA, contiguous, one floating dtype (float32 or float64), batch divisible by min(batch, im2col_step)."""
+    dtype = tensors[0][0].dtype
+    if dtype not in (torch.float32, torch.float64):
+        raise OdiseError(f"value: expected float32 or float64, got {dtype}")
+    for t, nm in tensors:
+        if not t.is_cuda:
+            raise OdiseError(f"{nm} must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise OdiseError(f"{nm} tensor has to be contiguous")
+        _req(t, dtype, nm)
+    N = tensors[0][0].shape[0]
+    step = min(N, im2col_step)
+    if step <= 0 or N % step != 0:
+        raise OdiseError(f"batch({N}) must divide im2col_step({step})")
+    return dtype
+
+
+def msda_forward_f64(value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step=128):
+    """msda_forward in float64 (the reference's AT_DISPATCH_FLOATING_TYPES double instantiation)."""
+    _msda_inputs(((value, "value"), (sampling_locations, "sampling_loc"), (attention_weights, "attn_weight")),
+                 im2col_step)
+    _req(value, torch.float64, "value")
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = sampling_locations.shape
+    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
+    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
+    out = torch.empty(N, Lq, M * D, dtype=torch.float64, device=value.device)
+    _check(load().odise_msda_forward_f64(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_locations),
+                                         _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P, _stream()),
+           "odise_msda_forward_f64")
+    return out
+
+
+def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=128):
+    """Drop-in for MSDA.ms_deform_attn_backward (reference ops/src/vision.cpp:20): same arguments, returns
+    [grad_value, grad_sampling_loc, grad_attn_weight] shaped like value / sampling_loc / attn_weight.  float32 or
+    float64 (all tensors of one dtype); RuntimeError on CPU, non-contiguous or mixed-dtype input and on a batch that
+    min(batch, im2col_step) does not divide.  The whole batch is one launch (im2col_step only checked)."""
+    dtype = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
+                          (grad_output, "grad_output")), im2col_step)
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = sampling_loc.shape
+    if grad_output.numel() != N * Lq * M * D:
+        raise OdiseError(f"grad_output: expected {N * Lq * M * D} elements, got {grad_output.numel()}")
+    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
+    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
+    grad_value = torch.empty_like(value)
+    grad_loc = torch.empty_like(sampling_loc)
+    grad_attn = torch.empty_like(attn_weight)
+    fn = "odise_msda_backward_f32" if dtype == torch.float32 else "odise_msda_backward_f64"
+    _check(getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output),
+                               _ptr(grad_value), _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P, _stream()), fn)
+    return [grad_value, grad_loc, grad_attn]
 
 
 class nvtx:
