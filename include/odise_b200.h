@@ -100,6 +100,18 @@ int odise_msda_fused_f32(const float* value, const int64_t* spatial_shapes, cons
                          const float* ref, const float* offs, const float* logits, float* out,
                          void* out_hi, void* out_lo, int N, int S, int M, int D, int L, int Lq, int P, void* stream);
 
+/* Backward of odise_msda_fused_f32 (inputs in its layouts, grad_out [N, Lq, M*D]): recomputes the locations and the
+ * softmax exactly as the forward does and writes
+ *   grad_value [N, S, M, D], grad_offs [N, Lq, M, L, P, 2] (gradient of the raw offsets), grad_logits [N, Lq, M, L*P]
+ * (all fully overwritten: grad_value is zero-filled on the stream, then accumulated with atomics).  The gradient of
+ * ref is grad_ref[n, q, l] = sum over (m, p) of grad_offs * (W_l, H_l), left to the caller.  D = 32 and L*P <= 32 only
+ * (ODISE_ERR_UNSUPPORTED otherwise).  No host synchronisation and no allocation (CUDA-graph capturable); grad_offs and
+ * grad_logits are bit-deterministic, grad_value depends on the order of the atomic reductions. */
+int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                  const float* ref, const float* offs, const float* logits, const float* grad_out,
+                                  float* grad_value, float* grad_offs, float* grad_logits,
+                                  int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * wgmma GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
  * Replaces F.conv2d / F.linear / torch.einsum call sites of the path (ldm ResBlock & attention linears via

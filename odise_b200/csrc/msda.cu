@@ -192,6 +192,50 @@ __device__ __forceinline__ MsdaCorners msda_corners(float lx, float ly, int H, i
   return c;
 }
 
+// Phase 1 of a (pair, sample) slot, shared by the D = 32 forward and backward kernels: the sample's level (H, W, start),
+// its location and its attention weight; a slot that is not live yields zeros.  FUSED = 1 computes
+// loc = ref + off / (W, H) and the softmax over the pair's L*P logits from the raw inputs, so the fused backward
+// differentiates exactly the bits its forward sampled with.  The softmax reduces over an aligned sub-warp of SL lanes
+// (slot = pair * SL + sample): every lane of the warp must make the call.
+struct MsdaSlot {
+  float lx, ly, aw;
+  int H, W, start;
+};
+
+template <int FUSED>
+__device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const float* __restrict__ loc_or_off,
+                                              const float* __restrict__ attn_or_logit, const float* __restrict__ ref,
+                                              long long pair, int s, bool live, int M, int L, int P, int SL) {
+  const int LP = L * P;
+  MsdaSlot r;
+  r.aw = 0.f; r.lx = 0.f; r.ly = 0.f;
+  r.H = 1; r.W = 1; r.start = 0;
+  if (live) {
+    const int l = s / P;
+    r.H = (int)__ldg(lv.shapes + 2 * l);
+    r.W = (int)__ldg(lv.shapes + 2 * l + 1);
+    r.start = (int)__ldg(lv.start + l);
+    const float2 xy = __ldg(reinterpret_cast<const float2*>(loc_or_off + (pair * LP + s) * 2));
+    r.aw = __ldg(attn_or_logit + pair * LP + s);
+    r.lx = xy.x; r.ly = xy.y;
+    if (FUSED) {
+      const long long nq = pair / M;
+      const float2 rp = __ldg(reinterpret_cast<const float2*>(ref + (nq * L + l) * 2));
+      r.lx = rp.x + xy.x / (float)r.W;        // ms_deform_attn.py:104-107
+      r.ly = rp.y + xy.y / (float)r.H;
+    }
+  }
+  if (FUSED) {                                 // softmax over the L*P logits of the pair (ms_deform_attn.py:100)
+    float mx = live ? r.aw : -INFINITY;
+    for (int o = SL >> 1; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const float e = live ? expf(r.aw - mx) : 0.f;
+    float sum = e;
+    for (int o = SL >> 1; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    r.aw = e / sum;
+  }
+  return r;
+}
+
 template <int FUSED>
 __global__ void __launch_bounds__(256)
 msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const float* __restrict__ loc_or_off,
@@ -211,33 +255,10 @@ msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const floa
     const int pl = slot / SL, s = slot - pl * SL;
     const long long pair = pair0 + pl;
     const bool live = (s < LP) && (pair < pairs);
-    float aw = 0.f, lx = 0.f, ly = 0.f;
-    int H = 1, W = 1, start = 0;
+    const MsdaSlot sl = msda_slot<FUSED>(lv, loc_or_off, attn_or_logit, ref, pair, s, live, M, L, P, SL);
     if (live) {
-      const int l = s / P;
-      H = (int)__ldg(lv.shapes + 2 * l);
-      W = (int)__ldg(lv.shapes + 2 * l + 1);
-      start = (int)__ldg(lv.start + l);
-      const float2 xy = __ldg(reinterpret_cast<const float2*>(loc_or_off + (pair * LP + s) * 2));
-      aw = __ldg(attn_or_logit + pair * LP + s);
-      lx = xy.x; ly = xy.y;
-      if (FUSED) {
-        const long long nq = pair / M;
-        const float2 r = __ldg(reinterpret_cast<const float2*>(ref + (nq * L + l) * 2));
-        lx = r.x + xy.x / (float)W;          // ms_deform_attn.py:104-107
-        ly = r.y + xy.y / (float)H;
-      }
-    }
-    if (FUSED) {                               // softmax over the L*P logits of the pair (ms_deform_attn.py:100)
-      float mx = live ? aw : -INFINITY;
-      for (int o = SL >> 1; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      const float e = live ? expf(aw - mx) : 0.f;
-      float sum = e;
-      for (int o = SL >> 1; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-      aw = e / sum;
-    }
-    if (live) {
-      const MsdaCorners cn = msda_corners(lx, ly, H, W, start, pix);
+      const float aw = sl.aw;
+      const MsdaCorners cn = msda_corners(sl.lx, sl.ly, sl.H, sl.W, sl.start, pix);
       s_off[pl * LP + s] = cn.off;
       s_w[pl * LP + s] = make_float4(cn.w.x * aw, cn.w.y * aw, cn.w.z * aw, cn.w.w * aw);
     }
@@ -313,11 +334,19 @@ __device__ __forceinline__ float dot4(const float4& a, const float4& b) {
 // the reference's scalar atomics).  The partials are summed over the 8 lanes with xor shuffles and one lane stores
 // grad_attn and grad_loc: no atomics there, so both are bit-deterministic; only grad_value depends on the order of the
 // reductions, as in the reference.
+//
+// FUSED = 1 is the backward of odise_msda_fused_f32: loc / attn are the raw offsets / logits (+ ref, SL as in the
+// forward).  Phase 1 recomputes location and softmax with the forward's msda_slot on the forward's slot layout.  Phase 2
+// writes grad_off = grad_loc / (W, H) = (attn * sw, attn * sh) (the W and H of grad_loc cancel) and keeps the
+// per-sample grad_attn partial sv in the slot's lh field, which is dead once every lane of the pair has read it; after
+// the loop grad_logit[s] = attn_s * (sv_s - sum_t attn_t * sv_t), the softmax backward, with the sum taken in sample
+// order in every lane.  grad_off and grad_logit are written without atomics and are bit-deterministic.
+template <int FUSED>
 __global__ void __launch_bounds__(256)
 msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, const float* __restrict__ loc,
                          const float* __restrict__ attn, const float* __restrict__ grad_out,
                          float* __restrict__ grad_value, float* __restrict__ grad_loc, float* __restrict__ grad_attn,
-                         int N, int S, int M, int L, int Lq, int P) {
+                         int N, int S, int M, int L, int Lq, int P, const float* __restrict__ ref, int SL) {
   extern __shared__ __align__(16) uint8_t msda_smem[];
   const int LP = L * P;
   int4* s_off = reinterpret_cast<int4*>(msda_smem);                                   // [PAIRS][LP]
@@ -328,24 +357,46 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
   const int pix = M * 32;
 
   // ---- phase 1: (pair, sample) slots; pairs past the end get zero corners so that their lanes do no memory work
-  for (int slot = threadIdx.x; slot < MSDA_PAIRS * LP; slot += 256) {
-    const int pl = slot / LP, s = slot - pl * LP;
-    const long long pair = pair0 + pl;
-    int4 o4 = make_int4(0, 0, 0, 0);
-    float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
-    if (pair < pairs) {
-      const int l = s / P;
-      const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
-      const int start = (int)__ldg(lv.start + l);
-      const float2 xy = __ldg(reinterpret_cast<const float2*>(loc + (pair * LP + s) * 2));
-      const MsdaCorners cn = msda_corners(xy.x, xy.y, H, W, start, pix);
-      o4 = cn.off;
-      w4 = cn.w;
-      f4 = make_float4(cn.lh, cn.lw, __ldg(attn + pair * LP + s), __int_as_float(cn.valid));
+  if (FUSED) {
+    for (int slot = threadIdx.x; slot < MSDA_PAIRS * SL; slot += 256) {
+      const int pl = slot / SL, s = slot - pl * SL;
+      const long long pair = pair0 + pl;
+      const bool live = (s < LP) && (pair < pairs);
+      const MsdaSlot sl = msda_slot<1>(lv, loc, attn, ref, pair, s, live, M, L, P, SL);
+      if (s < LP) {
+        int4 o4 = make_int4(0, 0, 0, 0);
+        float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
+        if (live) {
+          const MsdaCorners cn = msda_corners(sl.lx, sl.ly, sl.H, sl.W, sl.start, pix);
+          o4 = cn.off;
+          w4 = cn.w;
+          f4 = make_float4(cn.lh, cn.lw, sl.aw, __int_as_float(cn.valid));
+        }
+        s_off[pl * LP + s] = o4;
+        s_w[pl * LP + s] = w4;
+        s_f[pl * LP + s] = f4;
+      }
     }
-    s_off[slot] = o4;
-    s_w[slot] = w4;
-    s_f[slot] = f4;
+  } else {
+    for (int slot = threadIdx.x; slot < MSDA_PAIRS * LP; slot += 256) {
+      const int pl = slot / LP, s = slot - pl * LP;
+      const long long pair = pair0 + pl;
+      int4 o4 = make_int4(0, 0, 0, 0);
+      float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
+      if (pair < pairs) {
+        const int l = s / P;
+        const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
+        const int start = (int)__ldg(lv.start + l);
+        const float2 xy = __ldg(reinterpret_cast<const float2*>(loc + (pair * LP + s) * 2));
+        const MsdaCorners cn = msda_corners(xy.x, xy.y, H, W, start, pix);
+        o4 = cn.off;
+        w4 = cn.w;
+        f4 = make_float4(cn.lh, cn.lw, __ldg(attn + pair * LP + s), __int_as_float(cn.valid));
+      }
+      s_off[slot] = o4;
+      s_w[slot] = w4;
+      s_f[slot] = f4;
+    }
   }
   __syncthreads();
 
@@ -363,7 +414,8 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
   const float4 g = live ? ld4(grad_out + pair * 32 + c) : zero;
   const int4* po = s_off + pl * LP;
   const float4* pw = s_w + pl * LP;
-  const float4* pf = s_f + pl * LP;
+  float4* pf = s_f + pl * LP;
+  float dot = 0.f;                                    // FUSED: sum_t attn_t * sv_t
   for (int l = 0, s = 0; l < L; ++l) {
     const float Hf = (float)__ldg(lv.shapes + 2 * l), Wf = (float)__ldg(lv.shapes + 2 * l + 1);
 #pragma unroll 2
@@ -397,10 +449,26 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
         sh += __shfl_xor_sync(0xffffffffu, sh, o);
         sw += __shfl_xor_sync(0xffffffffu, sw, o);
       }
-      if (live && c == 0) {
+      if (FUSED) {
+        __syncwarp();                                 // all lanes of the pair have read pf[s]: its lh is dead
+        if (live && c == 0) {
+          *reinterpret_cast<float2*>(grad_loc + 2 * (pair * LP + s)) = make_float2(aw * sw, aw * sh);
+          pf[s].x = sv;
+        }
+        dot = fmaf(aw, sv, dot);
+      } else if (live && c == 0) {
         const long long i = pair * LP + s;
         grad_attn[i] = sv;
         *reinterpret_cast<float2*>(grad_loc + 2 * i) = make_float2(Wf * aw * sw, Hf * aw * sh);
+      }
+    }
+  }
+  if (FUSED) {                                        // softmax backward: the 8 lanes of a pair split its samples
+    __syncwarp();
+    if (live) {
+      for (int s = threadIdx.x & 7; s < LP; s += 8) {
+        const float4 f4 = pf[s];
+        grad_attn[pair * LP + s] = f4.z * (f4.x - dot);
       }
     }
   }
@@ -530,8 +598,8 @@ static int msda_backward(const T* value, const int64_t* spatial_shapes, const in
       // 48 B of shared memory per (pair, sample): at most 32 x 32 x 48 = 48 KB, the default dynamic limit
       const size_t smem = (size_t)MSDA_PAIRS * L * P * (sizeof(int4) + 2 * sizeof(float4));
       const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
-      msda_d32_backward_kernel<<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value, grad_loc,
-                                                              grad_attn, N, S, M, L, Lq, P);
+      msda_d32_backward_kernel<0><<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value, grad_loc,
+                                                                 grad_attn, N, S, M, L, Lq, P, nullptr, 1);
       d32 = true;
     }
   }
@@ -579,6 +647,35 @@ extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_s
                                                     reinterpret_cast<__nv_bfloat16*>(out_hi),
                                                     lo_arg(reinterpret_cast<__nv_bfloat16*>(out_lo)), N, S, M, D, L, Lq, P, lph);
   }
+  count_launch(1);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes,
+                                             const int64_t* level_start, const float* ref, const float* offs,
+                                             const float* logits, const float* grad_out, float* grad_value,
+                                             float* grad_offs, float* grad_logits, int N, int S, int M, int D, int L,
+                                             int Lq, int P, void* stream_v) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  if (!value || !spatial_shapes || !level_start || !ref || !offs || !logits || !grad_out || !grad_value || !grad_offs ||
+      !grad_logits)
+    return ODISE_ERR_ARG;
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  if (!d32_ok(S, M, D, L, P)) return ODISE_ERR_UNSUPPORTED;
+  const long long pairs = (long long)N * Lq * M;
+  const long long blocks = (pairs + MSDA_PAIRS - 1) / MSDA_PAIRS;
+  if (blocks > 0x7fffffffLL) return ODISE_ERR_ARG;
+  MsdaLevels lv{spatial_shapes, level_start};
+  cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(float) * (size_t)N * S * M * D, stream);
+  if (e != cudaSuccess) return (int)e;
+  const int LP = L * P;
+  int SL = 1;
+  while (SL < LP) SL <<= 1;
+  // 48 B of shared memory per (pair, sample), as in the non-fused backward: at most 48 KB at L*P = 32
+  const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + 2 * sizeof(float4));
+  msda_d32_backward_kernel<1><<<(unsigned)blocks, 256, smem, stream>>>(value, lv, offs, logits, grad_out, grad_value,
+                                                                       grad_offs, grad_logits, N, S, M, L, Lq, P, ref,
+                                                                       SL);
   count_launch(1);
   return (int)cudaGetLastError();
 }

@@ -52,6 +52,7 @@ _SIGS = {
     "odise_msda_forward_f64": [c_void_p] * 6 + [c_int] * 7 + [c_void_p],
     "odise_msda_backward_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
     "odise_msda_backward_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_backward_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -521,6 +522,72 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     _check(getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output),
                                _ptr(grad_value), _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P, _stream()), fn)
     return [grad_value, grad_loc, grad_attn]
+
+
+ODISE_ERR_UNSUPPORTED = 10006
+
+
+def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None):
+    """Checks of the fused entry points: CUDA, contiguous, float32, and the layouts of odise_msda_fused_f32
+    (value [N, S, M, D], reference_points [N, Lq, L, 2], offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P],
+    grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P, spatial_shapes, level_start_index) with the two index tensors
+    as int64 on the value's device."""
+    named = [(value, "value"), (reference_points, "reference_points"), (offsets, "offsets"), (logits, "logits")]
+    if grad_output is not None:
+        named.append((grad_output, "grad_output"))
+    for t, nm in named:
+        if not t.is_cuda:
+            raise OdiseError(f"{nm} must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise OdiseError(f"{nm} tensor has to be contiguous")
+        _req(t, torch.float32, nm)
+    if value.dim() != 4 or offsets.dim() != 6:
+        raise OdiseError(f"value must be [N, S, M, D] and offsets [N, Lq, M, L, P, 2], got {tuple(value.shape)} and "
+                         f"{tuple(offsets.shape)}")
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = offsets.shape
+    want = {"offsets": (N, Lq, M, L, P, 2), "reference_points": (N, Lq, L, 2), "logits": (N, Lq, M, L * P),
+            "spatial_shapes": (L, 2), "level_start_index": (L,)}
+    if grad_output is not None:
+        want["grad_output"] = (N, Lq, M * D)
+    for t, nm in named[1:] + [(spatial_shapes, "spatial_shapes"), (level_start_index, "level_start_index")]:
+        if tuple(t.shape) != want[nm]:
+            raise OdiseError(f"{nm}: expected shape {want[nm]}, got {tuple(t.shape)}")
+    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
+    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
+    return N, S, M, D, L, Lq, P, ss, ls
+
+
+def msda_fused_forward(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+    """MSDeformAttn's sampling from the raw linear outputs (odise_msda_fused_f32: softmax over L*P and
+    loc = ref + off / (W_l, H_l) inside the kernel) -> out [N, Lq, M*D] float32.  RuntimeError on CPU, non-contiguous or
+    non-float32 tensors, on shapes that disagree and on a D the kernel does not take."""
+    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
+                                                      offsets, logits)
+    out = torch.empty(N, Lq, M * D, dtype=torch.float32, device=value.device)
+    _check(load().odise_msda_fused_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
+                                       _ptr(logits), _ptr(out), None, None, N, S, M, D, L, Lq, P, _stream()),
+           "odise_msda_fused_f32")
+    return out
+
+
+def msda_fused_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output):
+    """Backward of msda_fused_forward (odise_msda_fused_backward_f32) -> (grad_value, grad_offsets, grad_logits) shaped
+    like value / offsets / logits.  D = 32 and L*P <= 32 only; RuntimeError otherwise and on the input errors of
+    msda_fused_forward.  grad_offsets and grad_logits are bit-deterministic."""
+    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
+                                                      offsets, logits, grad_output)
+    grad_value = torch.empty_like(value)
+    grad_offs = torch.empty_like(offsets)
+    grad_logits = torch.empty_like(logits)
+    rc = load().odise_msda_fused_backward_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
+                                              _ptr(logits), _ptr(grad_output), _ptr(grad_value), _ptr(grad_offs),
+                                              _ptr(grad_logits), N, S, M, D, L, Lq, P, _stream())
+    if rc == ODISE_ERR_UNSUPPORTED:
+        raise OdiseError(f"odise_msda_fused_backward_f32: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and "
+                         "S*M*D < 2^31 only)")
+    _check(rc, "odise_msda_fused_backward_f32")
+    return grad_value, grad_offs, grad_logits
 
 
 class nvtx:
