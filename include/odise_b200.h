@@ -112,6 +112,30 @@ int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_sha
                                   float* grad_value, float* grad_offs, float* grad_logits,
                                   int N, int S, int M, int D, int L, int Lq, int P, void* stream);
 
+/* The fused forward and backward with 16-bit storage (MSDeformAttn under torch.autocast or in a half / bfloat16 module):
+ * _f16 takes IEEE binary16 (__half), _bf16 takes bfloat16.  value, offs, logits, grad_out, out, grad_offs and grad_logits
+ * are in that type; ref stays float32 (the location's precision depends on it); grad_value is a float32 buffer
+ * [N, S, M, D], zero-filled on the stream and accumulated with fp32 atomics (the caller rounds it once if it wants the
+ * 16-bit type).  Every 16-bit load is converted to float exactly, all arithmetic is the float32 kernels' in the same
+ * order, and every 16-bit output is one round-to-nearest-even of the float32 result: out, grad_offs and grad_logits equal
+ * the _f32 entry points' results on the upcast inputs, rounded.  D = 32, L*P <= 32 and S*M*D < 2^31 only
+ * (ODISE_ERR_UNSUPPORTED otherwise, in both directions).  No host synchronisation and no allocation (CUDA-graph
+ * capturable); grad_offs and grad_logits are bit-deterministic, grad_value depends on the order of the atomics. */
+int odise_msda_fused_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                         const float* ref, const void* offs, const void* logits, void* out,
+                         int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                          const float* ref, const void* offs, const void* logits, void* out,
+                          int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_backward_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                  const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                  float* grad_value, void* grad_offs, void* grad_logits,
+                                  int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_backward_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                   const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                   float* grad_value, void* grad_offs, void* grad_logits,
+                                   int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * wgmma GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
  * Replaces F.conv2d / F.linear / torch.einsum call sites of the path (ldm ResBlock & attention linears via

@@ -24,6 +24,51 @@ struct MsdaLevels {
 };
 
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+
+// Storage-type loads and stores of the D = 32 fused kernels (float, or 16-bit __half / __nv_bfloat16 under autocast).
+// A 16-bit load converts to float right after it (exact); a 16-bit store rounds the fp32 result once (round to nearest
+// even).  Everything in between is fp32.  Four 16-bit channels are one 64-bit load / store.
+__device__ __forceinline__ float4 ld4(const __half* p) {
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) {
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
+  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float2 ld2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
+__device__ __forceinline__ float2 ld2(const __half* p) { return __half22float2(__ldg(reinterpret_cast<const __half2*>(p))); }
+__device__ __forceinline__ float2 ld2(const __nv_bfloat16* p) {
+  return __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(p)));
+}
+__device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld1(const __half* p) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float ld1(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void st4(__half* p, float4 v) {
+  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+}
+__device__ __forceinline__ void st4(__nv_bfloat16* p, float4 v) {
+  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+}
+__device__ __forceinline__ void st2(float* p, float2 v) { *reinterpret_cast<float2*>(p) = v; }
+__device__ __forceinline__ void st2(__half* p, float2 v) {
+  *reinterpret_cast<__half2*>(p) = __floats2half2_rn(v.x, v.y);
+}
+__device__ __forceinline__ void st2(__nv_bfloat16* p, float2 v) {
+  *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(v.x, v.y);
+}
+__device__ __forceinline__ void st1(float* p, float v) { *p = v; }
+__device__ __forceinline__ void st1(__half* p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void st1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
+
 __device__ __forceinline__ void fma4(float4& acc, float w, const float4& v) {
   acc.x = fmaf(w, v.x, acc.x); acc.y = fmaf(w, v.y, acc.y); acc.z = fmaf(w, v.z, acc.z); acc.w = fmaf(w, v.w, acc.w);
 }
@@ -196,15 +241,16 @@ __device__ __forceinline__ MsdaCorners msda_corners(float lx, float ly, int H, i
 // its location and its attention weight; a slot that is not live yields zeros.  FUSED = 1 computes
 // loc = ref + off / (W, H) and the softmax over the pair's L*P logits from the raw inputs, so the fused backward
 // differentiates exactly the bits its forward sampled with.  The softmax reduces over an aligned sub-warp of SL lanes
-// (slot = pair * SL + sample): every lane of the warp must make the call.
+// (slot = pair * SL + sample): every lane of the warp must make the call.  T is the storage type of the offsets and
+// logits (float, or 16-bit with FUSED = 1); they are converted to float as they are loaded, ref is always float.
 struct MsdaSlot {
   float lx, ly, aw;
   int H, W, start;
 };
 
-template <int FUSED>
-__device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const float* __restrict__ loc_or_off,
-                                              const float* __restrict__ attn_or_logit, const float* __restrict__ ref,
+template <int FUSED, typename T>
+__device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const T* __restrict__ loc_or_off,
+                                              const T* __restrict__ attn_or_logit, const float* __restrict__ ref,
                                               long long pair, int s, bool live, int M, int L, int P, int SL) {
   const int LP = L * P;
   MsdaSlot r;
@@ -215,8 +261,8 @@ __device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const float*
     r.H = (int)__ldg(lv.shapes + 2 * l);
     r.W = (int)__ldg(lv.shapes + 2 * l + 1);
     r.start = (int)__ldg(lv.start + l);
-    const float2 xy = __ldg(reinterpret_cast<const float2*>(loc_or_off + (pair * LP + s) * 2));
-    r.aw = __ldg(attn_or_logit + pair * LP + s);
+    const float2 xy = ld2(loc_or_off + (pair * LP + s) * 2);
+    r.aw = ld1(attn_or_logit + pair * LP + s);
     r.lx = xy.x; r.ly = xy.y;
     if (FUSED) {
       const long long nq = pair / M;
@@ -236,10 +282,12 @@ __device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const float*
   return r;
 }
 
-template <int FUSED>
+// T: storage type of value, loc_or_off, attn_or_logit and out.  float for both FUSED; __half / __nv_bfloat16 with
+// FUSED = 1 (odise_msda_fused_f16 / _bf16: a lane's 4 channels are one 64-bit load per corner, out_hi / out_lo unused).
+template <int FUSED, typename T>
 __global__ void __launch_bounds__(256)
-msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const float* __restrict__ loc_or_off,
-                const float* __restrict__ attn_or_logit, const float* __restrict__ ref, float* __restrict__ out,
+msda_d32_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc_or_off,
+                const T* __restrict__ attn_or_logit, const float* __restrict__ ref, T* __restrict__ out,
                 __nv_bfloat16* __restrict__ out_hi, __nv_bfloat16* __restrict__ out_lo, int N, int S, int M, int L,
                 int Lq, int P, int SL /* pow2 >= L*P, <= 32 */) {
   extern __shared__ __align__(16) uint8_t msda_smem[];
@@ -255,7 +303,7 @@ msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const floa
     const int pl = slot / SL, s = slot - pl * SL;
     const long long pair = pair0 + pl;
     const bool live = (s < LP) && (pair < pairs);
-    const MsdaSlot sl = msda_slot<FUSED>(lv, loc_or_off, attn_or_logit, ref, pair, s, live, M, L, P, SL);
+    const MsdaSlot sl = msda_slot<FUSED, T>(lv, loc_or_off, attn_or_logit, ref, pair, s, live, M, L, P, SL);
     if (live) {
       const float aw = sl.aw;
       const MsdaCorners cn = msda_corners(sl.lx, sl.ly, sl.H, sl.W, sl.start, pix);
@@ -272,7 +320,7 @@ msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const floa
   const int c = (threadIdx.x & 7) * 4;
   const int m = (int)(pair % M);
   const int n = (int)(pair / M / Lq);
-  const float* vb = value + (long long)n * S * pix + m * 32 + c;
+  const T* vb = value + (long long)n * S * pix + m * 32 + c;
   const int4* po = s_off + pl * LP;
   const float4* pw = s_w + pl * LP;
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -284,7 +332,7 @@ msda_d32_kernel(const float* __restrict__ value, const MsdaLevels lv, const floa
     fma4(acc, w4.x, v1); fma4(acc, w4.y, v2); fma4(acc, w4.z, v3); fma4(acc, w4.w, v4);
   }
   const long long o = pair * 32 + c;
-  if (out) *reinterpret_cast<float4*>(out + o) = acc;
+  if (out) st4(out + o, acc);
   if (out_hi) {
     const float e[4] = {acc.x, acc.y, acc.z, acc.w};
     store_planes<4>(out_hi + o, out_lo ? out_lo + o : nullptr, e);
@@ -296,9 +344,9 @@ static bool d32_ok(int S, int M, int D, int L, int P) {
   return D == 32 && L * P <= 32 && (long long)S * M * D < (1LL << 31);
 }
 
-template <int FUSED>
-static void launch_d32(const float* value, const MsdaLevels& lv, const float* a, const float* b, const float* ref,
-                       float* out, __nv_bfloat16* hi, __nv_bfloat16* lo, int N, int S, int M, int L, int Lq, int P,
+template <int FUSED, typename T>
+static void launch_d32(const T* value, const MsdaLevels& lv, const T* a, const T* b, const float* ref,
+                       T* out, __nv_bfloat16* hi, __nv_bfloat16* lo, int N, int S, int M, int L, int Lq, int P,
                        cudaStream_t stream) {
   const int LP = L * P;
   int SL = 1;
@@ -306,7 +354,7 @@ static void launch_d32(const float* value, const MsdaLevels& lv, const float* a,
   const long long pairs = (long long)N * Lq * M;
   const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
   const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + sizeof(float4));
-  msda_d32_kernel<FUSED><<<blocks, 256, smem, stream>>>(value, lv, a, b, ref, out, hi, lo, N, S, M, L, Lq, P, SL);
+  msda_d32_kernel<FUSED, T><<<blocks, 256, smem, stream>>>(value, lv, a, b, ref, out, hi, lo, N, S, M, L, Lq, P, SL);
 }
 
 static bool vec_ok(int D) { return D % 4 == 0 && D <= 128 && (32 % (D / 4) == 0); }
@@ -341,11 +389,15 @@ __device__ __forceinline__ float dot4(const float4& a, const float4& b) {
 // per-sample grad_attn partial sv in the slot's lh field, which is dead once every lane of the pair has read it; after
 // the loop grad_logit[s] = attn_s * (sv_s - sum_t attn_t * sv_t), the softmax backward, with the sum taken in sample
 // order in every lane.  grad_off and grad_logit are written without atomics and are bit-deterministic.
-template <int FUSED>
+//
+// T: storage type of value, loc, attn, grad_out, grad_loc and grad_attn (float; __half / __nv_bfloat16 with FUSED = 1).
+// grad_value is float for every T: at the 1024^2 shape an element of the coarsest level takes hundreds of contributions,
+// which a 16-bit running sum would lose, so the caller rounds the fp32 sum once.
+template <int FUSED, typename T>
 __global__ void __launch_bounds__(256)
-msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, const float* __restrict__ loc,
-                         const float* __restrict__ attn, const float* __restrict__ grad_out,
-                         float* __restrict__ grad_value, float* __restrict__ grad_loc, float* __restrict__ grad_attn,
+msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc,
+                         const T* __restrict__ attn, const T* __restrict__ grad_out,
+                         float* __restrict__ grad_value, T* __restrict__ grad_loc, T* __restrict__ grad_attn,
                          int N, int S, int M, int L, int Lq, int P, const float* __restrict__ ref, int SL) {
   extern __shared__ __align__(16) uint8_t msda_smem[];
   const int LP = L * P;
@@ -362,7 +414,7 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
       const int pl = slot / SL, s = slot - pl * SL;
       const long long pair = pair0 + pl;
       const bool live = (s < LP) && (pair < pairs);
-      const MsdaSlot sl = msda_slot<1>(lv, loc, attn, ref, pair, s, live, M, L, P, SL);
+      const MsdaSlot sl = msda_slot<1, T>(lv, loc, attn, ref, pair, s, live, M, L, P, SL);
       if (s < LP) {
         int4 o4 = make_int4(0, 0, 0, 0);
         float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
@@ -387,11 +439,11 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
         const int l = s / P;
         const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
         const int start = (int)__ldg(lv.start + l);
-        const float2 xy = __ldg(reinterpret_cast<const float2*>(loc + (pair * LP + s) * 2));
+        const float2 xy = ld2(loc + (pair * LP + s) * 2);
         const MsdaCorners cn = msda_corners(xy.x, xy.y, H, W, start, pix);
         o4 = cn.off;
         w4 = cn.w;
-        f4 = make_float4(cn.lh, cn.lw, __ldg(attn + pair * LP + s), __int_as_float(cn.valid));
+        f4 = make_float4(cn.lh, cn.lw, ld1(attn + pair * LP + s), __int_as_float(cn.valid));
       }
       s_off[slot] = o4;
       s_w[slot] = w4;
@@ -408,7 +460,7 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
   const int m = (int)(pair % M);
   const int n = (int)(pair / M / Lq);
   const long long vbase = (long long)n * S * pix + m * 32 + c;
-  const float* vb = value + vbase;
+  const T* vb = value + vbase;
   float* gvb = grad_value + vbase;
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
   const float4 g = live ? ld4(grad_out + pair * 32 + c) : zero;
@@ -452,14 +504,14 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
       if (FUSED) {
         __syncwarp();                                 // all lanes of the pair have read pf[s]: its lh is dead
         if (live && c == 0) {
-          *reinterpret_cast<float2*>(grad_loc + 2 * (pair * LP + s)) = make_float2(aw * sw, aw * sh);
+          st2(grad_loc + 2 * (pair * LP + s), make_float2(aw * sw, aw * sh));
           pf[s].x = sv;
         }
         dot = fmaf(aw, sv, dot);
       } else if (live && c == 0) {
         const long long i = pair * LP + s;
-        grad_attn[i] = sv;
-        *reinterpret_cast<float2*>(grad_loc + 2 * i) = make_float2(Wf * aw * sw, Hf * aw * sh);
+        st1(grad_attn + i, sv);
+        st2(grad_loc + 2 * i, make_float2(Wf * aw * sw, Hf * aw * sh));
       }
     }
   }
@@ -468,7 +520,7 @@ msda_d32_backward_kernel(const float* __restrict__ value, const MsdaLevels lv, c
     if (live) {
       for (int s = threadIdx.x & 7; s < LP; s += 8) {
         const float4 f4 = pf[s];
-        grad_attn[pair * LP + s] = f4.z * (f4.x - dot);
+        st1(grad_attn + pair * LP + s, f4.z * (f4.x - dot));
       }
     }
   }
@@ -598,8 +650,9 @@ static int msda_backward(const T* value, const int64_t* spatial_shapes, const in
       // 48 B of shared memory per (pair, sample): at most 32 x 32 x 48 = 48 KB, the default dynamic limit
       const size_t smem = (size_t)MSDA_PAIRS * L * P * (sizeof(int4) + 2 * sizeof(float4));
       const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
-      msda_d32_backward_kernel<0><<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value, grad_loc,
-                                                                 grad_attn, N, S, M, L, Lq, P, nullptr, 1);
+      msda_d32_backward_kernel<0, float><<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value,
+                                                                        grad_loc, grad_attn, N, S, M, L, Lq, P, nullptr,
+                                                                        1);
       d32 = true;
     }
   }
@@ -651,11 +704,42 @@ extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_s
   return (int)cudaGetLastError();
 }
 
-extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes,
-                                             const int64_t* level_start, const float* ref, const float* offs,
-                                             const float* logits, const float* grad_out, float* grad_value,
-                                             float* grad_offs, float* grad_logits, int N, int S, int M, int D, int L,
-                                             int Lq, int P, void* stream_v) {
+// The fused forward in a 16-bit storage type T (odise_msda_fused_f16 / _bf16): D = 32 kernel only, no planes.
+template <typename T>
+static int msda_fused_16(const void* value_v, const int64_t* spatial_shapes, const int64_t* level_start,
+                         const float* ref, const void* offs_v, const void* logits_v, void* out_v, int N, int S, int M,
+                         int D, int L, int Lq, int P, void* stream_v) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  if (!value_v || !spatial_shapes || !level_start || !ref || !offs_v || !logits_v || !out_v) return ODISE_ERR_ARG;
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  if (!d32_ok(S, M, D, L, P)) return ODISE_ERR_UNSUPPORTED;
+  if (((long long)N * Lq * M + MSDA_PAIRS - 1) / MSDA_PAIRS > 0x7fffffffLL) return ODISE_ERR_ARG;
+  MsdaLevels lv{spatial_shapes, level_start};
+  launch_d32<1, T>(static_cast<const T*>(value_v), lv, static_cast<const T*>(offs_v), static_cast<const T*>(logits_v),
+                   ref, static_cast<T*>(out_v), nullptr, nullptr, N, S, M, L, Lq, P, stream);
+  count_launch(1);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int odise_msda_fused_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                    const float* ref, const void* offs, const void* logits, void* out, int N, int S,
+                                    int M, int D, int L, int Lq, int P, void* stream) {
+  return msda_fused_16<__half>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P, stream);
+}
+
+extern "C" int odise_msda_fused_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                     const float* ref, const void* offs, const void* logits, void* out, int N, int S,
+                                     int M, int D, int L, int Lq, int P, void* stream) {
+  return msda_fused_16<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
+                                      stream);
+}
+
+// The fused backward for storage type T; grad_value is an fp32 buffer for every T.
+template <typename T>
+static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                               const float* ref, const T* offs, const T* logits, const T* grad_out, float* grad_value,
+                               T* grad_offs, T* grad_logits, int N, int S, int M, int D, int L, int Lq, int P,
+                               void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value || !spatial_shapes || !level_start || !ref || !offs || !logits || !grad_out || !grad_value || !grad_offs ||
       !grad_logits)
@@ -673,9 +757,42 @@ extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* 
   while (SL < LP) SL <<= 1;
   // 48 B of shared memory per (pair, sample), as in the non-fused backward: at most 48 KB at L*P = 32
   const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + 2 * sizeof(float4));
-  msda_d32_backward_kernel<1><<<(unsigned)blocks, 256, smem, stream>>>(value, lv, offs, logits, grad_out, grad_value,
-                                                                       grad_offs, grad_logits, N, S, M, L, Lq, P, ref,
-                                                                       SL);
+  msda_d32_backward_kernel<1, T><<<(unsigned)blocks, 256, smem, stream>>>(value, lv, offs, logits, grad_out, grad_value,
+                                                                          grad_offs, grad_logits, N, S, M, L, Lq, P,
+                                                                          ref, SL);
   count_launch(1);
   return (int)cudaGetLastError();
+}
+
+extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes,
+                                             const int64_t* level_start, const float* ref, const float* offs,
+                                             const float* logits, const float* grad_out, float* grad_value,
+                                             float* grad_offs, float* grad_logits, int N, int S, int M, int D, int L,
+                                             int Lq, int P, void* stream) {
+  return msda_fused_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, stream);
+}
+
+extern "C" int odise_msda_fused_backward_f16(const void* value, const int64_t* spatial_shapes,
+                                             const int64_t* level_start, const float* ref, const void* offs,
+                                             const void* logits, const void* grad_out, float* grad_value,
+                                             void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                             int Lq, int P, void* stream) {
+  using T = __half;
+  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
+                                static_cast<const T*>(offs), static_cast<const T*>(logits),
+                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
+                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, stream);
+}
+
+extern "C" int odise_msda_fused_backward_bf16(const void* value, const int64_t* spatial_shapes,
+                                              const int64_t* level_start, const float* ref, const void* offs,
+                                              const void* logits, const void* grad_out, float* grad_value,
+                                              void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                              int Lq, int P, void* stream) {
+  using T = __nv_bfloat16;
+  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
+                                static_cast<const T*>(offs), static_cast<const T*>(logits),
+                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
+                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, stream);
 }

@@ -53,6 +53,10 @@ _SIGS = {
     "odise_msda_backward_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
     "odise_msda_backward_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
     "odise_msda_fused_backward_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_f16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_bf16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_backward_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_backward_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -527,11 +531,12 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
 ODISE_ERR_UNSUPPORTED = 10006
 
 
-def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None):
-    """Checks of the fused entry points: CUDA, contiguous, float32, and the layouts of odise_msda_fused_f32
-    (value [N, S, M, D], reference_points [N, Lq, L, 2], offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P],
-    grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P, spatial_shapes, level_start_index) with the two index tensors
-    as int64 on the value's device."""
+def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
+                       dtype=torch.float32):
+    """Checks of the fused entry points: CUDA, contiguous, reference_points float32 and every other tensor of `dtype`,
+    and the layouts of odise_msda_fused_f32 (value [N, S, M, D], reference_points [N, Lq, L, 2], offsets
+    [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P], grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P, spatial_shapes,
+    level_start_index) with the two index tensors as int64 on the value's device."""
     named = [(value, "value"), (reference_points, "reference_points"), (offsets, "offsets"), (logits, "logits")]
     if grad_output is not None:
         named.append((grad_output, "grad_output"))
@@ -540,7 +545,7 @@ def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_point
             raise OdiseError(f"{nm} must be a CUDA tensor")
         if not t.is_contiguous():
             raise OdiseError(f"{nm} tensor has to be contiguous")
-        _req(t, torch.float32, nm)
+        _req(t, torch.float32 if nm == "reference_points" else dtype, nm)
     if value.dim() != 4 or offsets.dim() != 6:
         raise OdiseError(f"value must be [N, S, M, D] and offsets [N, Lq, M, L, P, 2], got {tuple(value.shape)} and "
                          f"{tuple(offsets.shape)}")
@@ -588,6 +593,57 @@ def msda_fused_backward(value, spatial_shapes, level_start_index, reference_poin
                          "S*M*D < 2^31 only)")
     _check(rc, "odise_msda_fused_backward_f32")
     return grad_value, grad_offs, grad_logits
+
+
+_MSDA_16BIT = {torch.float16: "f16", torch.bfloat16: "bf16"}
+
+
+def _msda_16bit_suffix(value):
+    if value.dtype not in _MSDA_16BIT:
+        raise OdiseError(f"value: expected float16 or bfloat16, got {value.dtype} (float32 takes msda_fused_forward / "
+                         "msda_fused_backward)")
+    return _MSDA_16BIT[value.dtype]
+
+
+def _msda_16bit_rc(rc, fn, D, L, P):
+    if rc == ODISE_ERR_UNSUPPORTED:
+        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
+    _check(rc, fn)
+
+
+def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+    """msda_fused_forward with 16-bit storage (odise_msda_fused_f16 / _bf16, chosen by value.dtype): value, offsets and
+    logits float16 or bfloat16 (one dtype), reference_points float32 -> out [N, Lq, M*D] in the value's dtype, one rounding
+    of the fp32 result.  D = 32 and L*P <= 32 only.  RuntimeError on CPU or non-contiguous tensors, on a float32 value,
+    on mixed dtypes, on shapes that disagree and on unsupported shapes."""
+    sfx = _msda_16bit_suffix(value)
+    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
+                                                      offsets, logits, dtype=value.dtype)
+    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
+    fn = "odise_msda_fused_" + sfx
+    rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
+                             _ptr(out), N, S, M, D, L, Lq, P, _stream())
+    _msda_16bit_rc(rc, fn, D, L, P)
+    return out
+
+
+def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output):
+    """Backward of msda_fused_forward_16bit (odise_msda_fused_backward_f16 / _bf16) -> (grad_value, grad_offsets,
+    grad_logits), each in the value's dtype.  grad_value is accumulated in a float32 buffer and rounded once here;
+    grad_offsets and grad_logits are rounded once in the kernel and are bit-deterministic.  grad_output has the value's
+    dtype.  Errors as msda_fused_forward_16bit."""
+    sfx = _msda_16bit_suffix(value)
+    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
+                                                      offsets, logits, grad_output, dtype=value.dtype)
+    grad_value = torch.empty(value.shape, dtype=torch.float32, device=value.device)
+    grad_offs = torch.empty_like(offsets)
+    grad_logits = torch.empty_like(logits)
+    fn = "odise_msda_fused_backward_" + sfx
+    rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
+                             _ptr(grad_output), _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P,
+                             _stream())
+    _msda_16bit_rc(rc, fn, D, L, P)
+    return grad_value.to(value.dtype), grad_offs, grad_logits
 
 
 class nvtx:

@@ -8,8 +8,9 @@ the autograd Function and the nn.Module).
 MSDA exposes the native module's two entry points with its arguments and results, for float32 and float64 CUDA tensors;
 MSDeformAttnFunction is the autograd Function of ops/functions/ms_deform_attn_func.py:32-49 on top of them.
 MSDeformAttnFusedFunction differentiates the fused op (odise_msda_fused_f32 / odise_msda_fused_backward_f32: softmax and
-sampling locations computed inside the kernels), and MSDeformAttn is the module of ops/modules/ms_deform_attn.py,
-which takes the fused op where it applies.  All of them run the library's sm_90a kernels; there is no CPU path."""
+sampling locations computed inside the kernels; float16 and bfloat16 storage under autocast), and MSDeformAttn is the
+module of ops/modules/ms_deform_attn.py, which takes the fused op where it applies.  All of them run the library's sm_90a
+kernels; there is no CPU path."""
 import math
 import warnings
 
@@ -62,18 +63,24 @@ class MSDeformAttnFunction(Function):
         return grad_value, None, None, grad_sampling_loc, grad_attn_weight, None
 
 
+_LOW = (torch.float16, torch.bfloat16)
+
+
 class MSDeformAttnFusedFunction(Function):
-    """Autograd through the fused op: forward odise_msda_fused_f32, backward odise_msda_fused_backward_f32.
+    """Autograd through the fused op: forward odise_msda_fused_f32, backward odise_msda_fused_backward_f32, or their
+    16-bit forms (odise_msda_fused_f16 / _bf16 and the backward) when value is float16 or bfloat16.
 
     Inputs: value [N, S, M, D], spatial_shapes [L, 2], level_start_index [L], reference_points [N, Lq, L, 2], offsets
     [N, Lq, M, L, P, 2] (raw output of the sampling_offsets linear) and logits [N, Lq, M, L*P] (raw output of the
-    attention_weights linear); float32 CUDA tensors, D = 32 and L*P <= 32 for the backward.  Gradients for value,
-    offsets and logits; for reference_points only when it requires one, as grad_ref[n, q, l] = sum over (m, p) of
-    grad_offsets * (W_l, H_l)."""
+    attention_weights linear); CUDA tensors, value / offsets / logits float32 or all of one 16-bit dtype,
+    reference_points float32; D = 32 and L*P <= 32 for the backward (and for the 16-bit forward).  Gradients for value,
+    offsets and logits in their dtype; for reference_points only when it requires one, as grad_ref[n, q, l] = sum over
+    (m, p) of grad_offsets * (W_l, H_l), computed in float32."""
 
     @staticmethod
     def forward(ctx, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
-        output = lib.msda_fused_forward(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+        fwd = lib.msda_fused_forward_16bit if value.dtype in _LOW else lib.msda_fused_forward
+        output = fwd(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
         ctx.save_for_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
         return output
 
@@ -81,12 +88,15 @@ class MSDeformAttnFusedFunction(Function):
     @once_differentiable
     def backward(ctx, grad_output):
         value, spatial_shapes, level_start_index, reference_points, offsets, logits = ctx.saved_tensors
-        grad_value, grad_offsets, grad_logits = lib.msda_fused_backward(
-            value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output.contiguous())
+        bwd = lib.msda_fused_backward_16bit if value.dtype in _LOW else lib.msda_fused_backward
+        grad_value, grad_offsets, grad_logits = bwd(
+            value, spatial_shapes, level_start_index, reference_points, offsets, logits,
+            grad_output.to(value.dtype).contiguous())
         grad_ref = None
         if ctx.needs_input_grad[3]:
-            wh = torch.stack([spatial_shapes[:, 1], spatial_shapes[:, 0]], -1).to(grad_offsets)
-            grad_ref = (grad_offsets * wh[None, None, None, :, None, :]).sum((2, 4))
+            go = grad_offsets.float()
+            wh = torch.stack([spatial_shapes[:, 1], spatial_shapes[:, 0]], -1).to(go)
+            grad_ref = (go * wh[None, None, None, :, None, :]).sum((2, 4))
         return grad_value, None, None, grad_ref, grad_offsets, grad_logits
 
 
@@ -104,7 +114,12 @@ class MSDeformAttn(nn.Module):
     kernel for their backward) for float32 CUDA inputs with 2-column reference points, D = d_model / n_heads = 32,
     n_levels * n_points <= 32 and S * d_model < 2^31.  Every other input (other D, float64, 4-column box reference
     points, or use_fused = False) takes the reference's composition: softmax and locations in torch ops, then
-    MSDeformAttnFunction.  CPU tensors raise: there is no CPU path."""
+    MSDeformAttnFunction.  CPU tensors raise: there is no CPU path.
+
+    Under torch.autocast, or in a module cast to float16 / bfloat16, value, offsets and logits come out of the Linears in
+    16 bits.  Where the fused conditions hold, the 16-bit fused kernels take them as they are (reference points cast to
+    float32, which is exact) and return the value's dtype.  Elsewhere the composition runs in float32 on upcast inputs
+    and its output is cast back to the value's dtype before output_proj, as the reference's grid_sample fallback does."""
 
     def __init__(self, d_model=256, n_levels=4, n_heads=8, n_points=4):
         super().__init__()
@@ -163,12 +178,19 @@ class MSDeformAttn(nn.Module):
         value = value.view(N, S, M, D)
         offsets = self.sampling_offsets(query).view(N, Lq, M, L, P, 2)
         logits = self.attention_weights(query).view(N, Lq, M, L * P)
-        fused = (self.use_fused and value.dtype == torch.float32 and reference_points.dtype == torch.float32
-                 and reference_points.shape[-1] == 2 and D == 32 and L * P <= 32 and S * M * D < 2 ** 31)
+        low = value.dtype in _LOW
+        # float32 needs float32 reference points; a 16-bit value takes them in float32 or 16 bits (cast exactly below)
+        ref_ok = reference_points.dtype in ((torch.float32,) + _LOW if low else (torch.float32,))
+        fused = (self.use_fused and (value.dtype == torch.float32 or low) and offsets.dtype == logits.dtype == value.dtype
+                 and ref_ok and reference_points.shape[-1] == 2 and D == 32 and L * P <= 32 and S * M * D < 2 ** 31)
         if fused:
             output = MSDeformAttnFusedFunction.apply(value, input_spatial_shapes, input_level_start_index,
-                                                     reference_points.contiguous(), offsets, logits)
+                                                     reference_points.to(torch.float32).contiguous(), offsets, logits)
         else:
+            out_dtype = value.dtype
+            if low:                    # sample in float32 (what the reference's grid_sample fallback does under autocast)
+                value, offsets, logits = value.float(), offsets.float(), logits.float()
+                reference_points = reference_points.float()
             attention_weights = F.softmax(logits, -1).view(N, Lq, M, L, P)
             if reference_points.shape[-1] == 2:
                 wh = torch.stack([input_spatial_shapes[..., 1], input_spatial_shapes[..., 0]], -1)
@@ -178,4 +200,6 @@ class MSDeformAttn(nn.Module):
                                       + offsets / P * reference_points[:, :, None, :, None, 2:] * 0.5)
             output = MSDeformAttnFunction.apply(value, input_spatial_shapes, input_level_start_index,
                                                 sampling_locations, attention_weights, self.im2col_step)
+            if low:
+                output = output.to(out_dtype)
         return self.output_proj(output)
