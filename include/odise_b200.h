@@ -136,6 +136,40 @@ int odise_msda_fused_backward_bf16(const void* value, const int64_t* spatial_sha
                                    float* grad_value, void* grad_offs, void* grad_logits,
                                    int N, int S, int M, int D, int L, int Lq, int P, void* stream);
 
+/* Deterministic twins of the five backward entry points (PyTorch's torch.use_deterministic_algorithms): the same
+ * arguments plus a workspace of odise_msda_det_workspace_bytes(N, S, M, D) bytes (any content; 8-byte aligned), and a
+ * grad_value whose bits depend only on the inputs, not on the order of the reductions.  The fused 16-bit twins take
+ * grad_value in the storage type.  Every other output is bit-equal to the default entry point's.
+ * grad_value is summed in int64 fixed point: per (image n, head m), with G = max |grad_out[n, :, m, :]|,
+ * A = max |attn[n, :, m, :, :]| (A = 1 on the fused paths), 2^e >= G * A and K = Lq * P, every contribution is scaled
+ * by 2^s, s = 61 - ceil(log2 K) - e, and rounded to an integer; a finalize pass writes sum * 2^-s in the output type.
+ * An element with k contributions is off by at most k * 2^(e + ceil(log2 K) - 62): an absolute error relative to
+ * G * A (below 2^-26 G * A at the 1024^2 shape), not a relative one per element as with float atomics; the fp64 twin has the
+ * same bound (meant for gradcheck).  If grad_out (or, non-fused, attn) holds an inf or NaN in slice (n, m), or a
+ * contribution is not finite, grad_value[n, :, m, :] is NaN; other slices are unaffected.  No host synchronisation and
+ * no allocation (CUDA-graph capturable); ODISE_ERR_WORKSPACE for a null workspace. */
+long long odise_msda_det_workspace_bytes(int N, int S, int M, int D);
+int odise_msda_backward_det_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                const float* loc, const float* attn, const float* grad_out,
+                                float* grad_value, float* grad_loc, float* grad_attn,
+                                int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
+int odise_msda_backward_det_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                const double* loc, const double* attn, const double* grad_out,
+                                double* grad_value, double* grad_loc, double* grad_attn,
+                                int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
+int odise_msda_fused_backward_det_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref, const float* offs, const float* logits, const float* grad_out,
+                                      float* grad_value, float* grad_offs, float* grad_logits,
+                                      int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
+int odise_msda_fused_backward_det_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                      void* grad_value, void* grad_offs, void* grad_logits,
+                                      int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
+int odise_msda_fused_backward_det_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                       const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                       void* grad_value, void* grad_offs, void* grad_logits,
+                                       int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * wgmma GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
  * Replaces F.conv2d / F.linear / torch.einsum call sites of the path (ldm ResBlock & attention linears via

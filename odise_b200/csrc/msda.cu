@@ -371,9 +371,80 @@ static bool vec_ok(int D) { return D % 4 == 0 && D <= 128 && (32 % (D / 4) == 0)
 __device__ __forceinline__ float4 scale4(const float4& v, float s) {
   return make_float4(v.x * s, v.y * s, v.z * s, v.w * s);
 }
+// The backward kernels' sums of products are written with explicit fmaf / fma: the default (atomic) and the fixed-point
+// instantiations share this arithmetic and must give the same bits, while an implicit contraction may associate a sum
+// differently in each instantiation.  The association is the one nvcc picked for the default instantiations, whose SASS
+// is unchanged by writing it out.
 __device__ __forceinline__ float dot4(const float4& a, const float4& b) {
-  return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+  return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
 }
+// bilinear value w1 v1 + w2 v2 + w3 v3 + w4 v4 and its derivatives d/dh = hw (v3 - v1) + lw (v4 - v2),
+// d/dw = hh (v2 - v1) + lh (v4 - v3), for float and double
+__device__ __forceinline__ float msda_fma(float a, float b, float c) { return fmaf(a, b, c); }
+__device__ __forceinline__ double msda_fma(double a, double b, double c) { return fma(a, b, c); }
+template <typename T>
+__device__ __forceinline__ T msda_bil(T w1, T w2, T w3, T w4, T v1, T v2, T v3, T v4) {
+  return msda_fma(w4, v4, msda_fma(w3, v3, msda_fma(w1, v1, w2 * v2)));
+}
+
+// Accumulation policies of grad_value in the backward kernels; only the corner reductions differ between them.
+// MsdaAtomicAcc: floating-point atomics into grad_value (the default: fast, bits depend on the order of the reductions).
+struct MsdaAtomicAcc {
+  static constexpr bool fixed = false;
+};
+
+// MsdaFixedAcc: int64 fixed point (the deterministic entry points).  Integer addition is associative, so the sums do not
+// depend on the order of the reductions.  Per (image n, head m), with G = max |grad_out[n, :, m, :]|, A = max
+// |attn[n, :, m, :, :]| (A = 1 on the fused paths, whose softmax weights are <= 1), e = clog2(G) + clog2(A) (so
+// 2^e >= G * A, without forming the product) and K = Lq * P (an element takes at most one contribution per
+// (query, point) of its level): s = 61 - ceil(log2 K) - e.  Every contribution g * (w * aw) is computed in the storage arithmetic as
+// the atomic path does, scaled by 2^s exactly (|.| <= 2^(61 - ceil(log2 K)) plus product rounding) and rounded to the
+// nearest integer, so every sum stays below 2^62.  A contribution that is not finite, or does not fit, marks the
+// (n, m) slice non-finite; the finalize pass writes NaN there.
+struct MsdaFixedAcc {
+  static constexpr bool fixed = true;
+  unsigned long long* sum;          // [N, S, M, D] two's-complement int64 sums, zero-filled
+  unsigned long long* gmax;         // [N * M] bits of max |grad_out| as a double (>= +inf bits: non-finite slice)
+  const unsigned long long* amax;   // [N * M] bits of max |attn| as a double (0 on the fused paths: A taken as 1)
+  int log2k;                        // ceil(log2(Lq * P))
+};
+
+// least e with 2^e >= x for a finite x > 0; 0 for x = 0 (so A = 0 and A = 1 give the same shift)
+__device__ __forceinline__ int msda_clog2(double x) {
+  int e;
+  const double f = frexp(x, &e);                      // x = f * 2^e, f in [0.5, 1)
+  return f == 0.5 ? e - 1 : (x == 0.0 ? 0 : e);
+}
+
+__device__ __forceinline__ int msda_fixed_shift(const MsdaFixedAcc& a, long long nm) {
+  const double G = __longlong_as_double((long long)a.gmax[nm]), A = __longlong_as_double((long long)a.amax[nm]);
+  return 61 - a.log2k - (msda_clog2(G) + msda_clog2(A));
+}
+
+// one contribution in fixed point: float c * 2^s in double (exact: sc = 2^s, |s| < 400 for float inputs), double
+// c through ldexp (any s); `bad` collects contributions that are not finite or exceed 2^62
+__device__ __forceinline__ unsigned long long msda_fixed(float c, double sc, int, bool& bad) {
+  const double d = (double)c * sc;
+  bad |= !(fabs(d) < 0x1p62);
+  return (unsigned long long)__double2ll_rn(d);
+}
+__device__ __forceinline__ unsigned long long msda_fixed(double c, double, int s, bool& bad) {
+  const double d = ldexp(c, s);
+  bad |= !(fabs(d) < 0x1p62);
+  return (unsigned long long)__double2ll_rn(d);
+}
+
+// channels p[0], p[8], p[16], p[24] of a D = 32 head: with lane j of a pair at p = corner + j, each of the four
+// reductions covers 64 contiguous bytes (8 channels) across the pair's 8 lanes, two 32-byte sectors
+__device__ __forceinline__ void msda_fixed_add4(unsigned long long* p, const float4& c, double sc, bool& bad) {
+  atomicAdd(p + 0, msda_fixed(c.x, sc, 0, bad));
+  atomicAdd(p + 8, msda_fixed(c.y, sc, 0, bad));
+  atomicAdd(p + 16, msda_fixed(c.z, sc, 0, bad));
+  atomicAdd(p + 24, msda_fixed(c.w, sc, 0, bad));
+}
+
+constexpr unsigned long long MSDA_NAN_BITS = 0x7ff8000000000000ull;   // a quiet NaN: above the bits of +inf
+constexpr unsigned long long MSDA_INF_BITS = 0x7ff0000000000000ull;
 
 // D = 32: the forward's block of MSDA_PAIRS pairs.  Phase 1 stores per (pair, sample) the corners of msda_corners with
 // their bits and the attention weight; phase 2 runs 8 lanes per pair with one float4 of channels each (grad_out loaded
@@ -393,12 +464,18 @@ __device__ __forceinline__ float dot4(const float4& a, const float4& b) {
 // T: storage type of value, loc, attn, grad_out, grad_loc and grad_attn (float; __half / __nv_bfloat16 with FUSED = 1).
 // grad_value is float for every T: at the 1024^2 shape an element of the coarsest level takes hundreds of contributions,
 // which a 16-bit running sum would lose, so the caller rounds the fp32 sum once.
-template <int FUSED, typename T>
+//
+// Acc = MsdaFixedAcc (the deterministic entry points): grad_value is unused; each valid corner takes four 64-bit
+// integer reductions into acc.sum instead of one 128-bit float reduction.  For them lane j of a pair holds a second,
+// interleaved copy of grad_out (channels j, j + 8, j + 16, j + 24), so that each reduction instruction of the pair's 8
+// lanes covers 64 contiguous bytes; the contributions are the same products, summed by other lanes.
+template <int FUSED, typename T, typename Acc = MsdaAtomicAcc>
 __global__ void __launch_bounds__(256)
 msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc,
                          const T* __restrict__ attn, const T* __restrict__ grad_out,
                          float* __restrict__ grad_value, T* __restrict__ grad_loc, T* __restrict__ grad_attn,
-                         int N, int S, int M, int L, int Lq, int P, const float* __restrict__ ref, int SL) {
+                         int N, int S, int M, int L, int Lq, int P, const float* __restrict__ ref, int SL,
+                         const Acc acc) {
   extern __shared__ __align__(16) uint8_t msda_smem[];
   const int LP = L * P;
   int4* s_off = reinterpret_cast<int4*>(msda_smem);                                   // [PAIRS][LP]
@@ -468,6 +545,16 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
   const float4* pw = s_w + pl * LP;
   float4* pf = s_f + pl * LP;
   float dot = 0.f;                                    // FUSED: sum_t attn_t * sv_t
+  double sc = 0.0;                                    // fixed point: 2^s of the pair's (n, m)
+  bool bad = false;
+  float4 gt = zero;                                   // fixed point: channels j, j + 8, j + 16, j + 24 of lane j
+  if constexpr (Acc::fixed) {
+    if (live) {
+      sc = ldexp(1.0, msda_fixed_shift(acc, (long long)n * M + m));
+      const T* gp = grad_out + pair * 32 + (threadIdx.x & 7);
+      gt = make_float4(ld1(gp), ld1(gp + 8), ld1(gp + 16), ld1(gp + 24));
+    }
+  }
   for (int l = 0, s = 0; l < L; ++l) {
     const float Hf = (float)__ldg(lv.shapes + 2 * l), Wf = (float)__ldg(lv.shapes + 2 * l + 1);
 #pragma unroll 2
@@ -479,10 +566,10 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
                    v3 = (valid & 4) ? ld4(vb + o4.z) : zero, v4 = (valid & 8) ? ld4(vb + o4.w) : zero;
       const float lh = f4.x, lw = f4.y, hh = 1.f - lh, hw = 1.f - lw, aw = f4.z;
       float4 bil, dh, dw;
-      bil.x = w4.x * v1.x + w4.y * v2.x + w4.z * v3.x + w4.w * v4.x;
-      bil.y = w4.x * v1.y + w4.y * v2.y + w4.z * v3.y + w4.w * v4.y;
-      bil.z = w4.x * v1.z + w4.y * v2.z + w4.z * v3.z + w4.w * v4.z;
-      bil.w = w4.x * v1.w + w4.y * v2.w + w4.z * v3.w + w4.w * v4.w;
+      bil.x = msda_bil(w4.x, w4.y, w4.z, w4.w, v1.x, v2.x, v3.x, v4.x);
+      bil.y = msda_bil(w4.x, w4.y, w4.z, w4.w, v1.y, v2.y, v3.y, v4.y);
+      bil.z = msda_bil(w4.x, w4.y, w4.z, w4.w, v1.z, v2.z, v3.z, v4.z);
+      bil.w = msda_bil(w4.x, w4.y, w4.z, w4.w, v1.w, v2.w, v3.w, v4.w);
       dh.x = hw * (v3.x - v1.x) + lw * (v4.x - v2.x);
       dh.y = hw * (v3.y - v1.y) + lw * (v4.y - v2.y);
       dh.z = hw * (v3.z - v1.z) + lw * (v4.z - v2.z);
@@ -492,10 +579,19 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
       dw.z = hh * (v2.z - v1.z) + lh * (v4.z - v3.z);
       dw.w = hh * (v2.w - v1.w) + lh * (v4.w - v3.w);
       float sv = dot4(g, bil), sh = dot4(g, dh), sw = dot4(g, dw);
-      if (valid & 1) atomicAdd(reinterpret_cast<float4*>(gvb + o4.x), scale4(g, w4.x * aw));
-      if (valid & 2) atomicAdd(reinterpret_cast<float4*>(gvb + o4.y), scale4(g, w4.y * aw));
-      if (valid & 4) atomicAdd(reinterpret_cast<float4*>(gvb + o4.z), scale4(g, w4.z * aw));
-      if (valid & 8) atomicAdd(reinterpret_cast<float4*>(gvb + o4.w), scale4(g, w4.w * aw));
+      if constexpr (Acc::fixed) {
+        // the same per-channel products g_c * (w * aw) as the atomic path, channels interleaved across the lanes
+        unsigned long long* sb = acc.sum + (vbase - c) + (threadIdx.x & 7);
+        if (valid & 1) msda_fixed_add4(sb + o4.x, scale4(gt, w4.x * aw), sc, bad);
+        if (valid & 2) msda_fixed_add4(sb + o4.y, scale4(gt, w4.y * aw), sc, bad);
+        if (valid & 4) msda_fixed_add4(sb + o4.z, scale4(gt, w4.z * aw), sc, bad);
+        if (valid & 8) msda_fixed_add4(sb + o4.w, scale4(gt, w4.w * aw), sc, bad);
+      } else {
+        if (valid & 1) atomicAdd(reinterpret_cast<float4*>(gvb + o4.x), scale4(g, w4.x * aw));
+        if (valid & 2) atomicAdd(reinterpret_cast<float4*>(gvb + o4.y), scale4(g, w4.y * aw));
+        if (valid & 4) atomicAdd(reinterpret_cast<float4*>(gvb + o4.z), scale4(g, w4.z * aw));
+        if (valid & 8) atomicAdd(reinterpret_cast<float4*>(gvb + o4.w), scale4(g, w4.w * aw));
+      }
       for (int o = 4; o; o >>= 1) {
         sv += __shfl_xor_sync(0xffffffffu, sv, o);
         sh += __shfl_xor_sync(0xffffffffu, sh, o);
@@ -524,17 +620,21 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
       }
     }
   }
+  if constexpr (Acc::fixed) {
+    if (bad) atomicMax(acc.gmax + (long long)n * M + m, MSDA_NAN_BITS);   // e.g. NaN softmax weights from NaN logits
+  }
 }
 
 // Generic path (any D, float or double, 64-bit offsets): one warp per (query, head) pair, lanes stride over the
 // channels, the three partials are summed with warp shuffles and lane 0 stores grad_attn / grad_loc.  grad_value takes
-// plain scalar atomics (native for double on sm_90).
-template <typename T>
+// plain scalar atomics (native for double on sm_90); with Acc = MsdaFixedAcc one 64-bit integer reduction per channel
+// into acc.sum.
+template <typename T, typename Acc = MsdaAtomicAcc>
 __global__ void __launch_bounds__(256)
 msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc,
                           const T* __restrict__ attn, const T* __restrict__ grad_out, T* __restrict__ grad_value,
                           T* __restrict__ grad_loc, T* __restrict__ grad_attn, int N, int S, int M, int D, int L,
-                          int Lq, int P) {
+                          int Lq, int P, const Acc acc) {
   const long long pair = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   if (pair >= (long long)N * Lq * M) return;        // whole warps leave together
   const int lane = threadIdx.x & 31;
@@ -545,6 +645,13 @@ msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, cons
   const T* vb = value + vbase;
   T* gvb = grad_value + vbase;
   const T* go = grad_out + pair * D;
+  int sh_fx = 0;                                     // fixed point: s and 2^s of the pair's (n, m)
+  double sc = 0.0;
+  bool bad = false;
+  if constexpr (Acc::fixed) {
+    sh_fx = msda_fixed_shift(acc, n * M + m);
+    sc = ldexp(1.0, sh_fx);
+  }
   for (int l = 0; l < L; ++l) {
     const int H = (int)__ldg(lv.shapes + 2 * l), W = (int)__ldg(lv.shapes + 2 * l + 1);
     const long long start = __ldg(lv.start + l);
@@ -563,11 +670,19 @@ msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, cons
         for (int c = lane; c < D; c += 32) {
           const T gc = go[c], ga = gc * aw;
           T v1 = 0, v2 = 0, v3 = 0, v4 = 0;
-          if (t && lf) { v1 = vb[o1 + c]; atomicAdd(gvb + o1 + c, w1 * ga); }
-          if (t && rt) { v2 = vb[o2 + c]; atomicAdd(gvb + o2 + c, w2 * ga); }
-          if (b && lf) { v3 = vb[o3 + c]; atomicAdd(gvb + o3 + c, w3 * ga); }
-          if (b && rt) { v4 = vb[o4 + c]; atomicAdd(gvb + o4 + c, w4 * ga); }
-          sv += gc * (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4);
+          if constexpr (Acc::fixed) {
+            unsigned long long* sb = acc.sum + vbase + c;
+            if (t && lf) { v1 = vb[o1 + c]; atomicAdd(sb + o1, msda_fixed(w1 * ga, sc, sh_fx, bad)); }
+            if (t && rt) { v2 = vb[o2 + c]; atomicAdd(sb + o2, msda_fixed(w2 * ga, sc, sh_fx, bad)); }
+            if (b && lf) { v3 = vb[o3 + c]; atomicAdd(sb + o3, msda_fixed(w3 * ga, sc, sh_fx, bad)); }
+            if (b && rt) { v4 = vb[o4 + c]; atomicAdd(sb + o4, msda_fixed(w4 * ga, sc, sh_fx, bad)); }
+          } else {
+            if (t && lf) { v1 = vb[o1 + c]; atomicAdd(gvb + o1 + c, w1 * ga); }
+            if (t && rt) { v2 = vb[o2 + c]; atomicAdd(gvb + o2 + c, w2 * ga); }
+            if (b && lf) { v3 = vb[o3 + c]; atomicAdd(gvb + o3 + c, w3 * ga); }
+            if (b && rt) { v4 = vb[o4 + c]; atomicAdd(gvb + o4 + c, w4 * ga); }
+          }
+          sv += gc * msda_bil(w1, w2, w3, w4, v1, v2, v3, v4);
           sh += gc * (hw * (v3 - v1) + lw * (v4 - v2));
           sw += gc * (hh * (v2 - v1) + lh * (v4 - v3));
         }
@@ -582,6 +697,65 @@ msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, cons
         grad_loc[2 * i] = (T)W * aw * sw;
         grad_loc[2 * i + 1] = (T)H * aw * sh;
       }
+    }
+  }
+  if constexpr (Acc::fixed) {
+    if (bad) atomicMax(acc.gmax + n * M + m, MSDA_NAN_BITS);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Deterministic backward: the passes around the fixed-point instantiations (MsdaFixedAcc above).
+
+// Pre-pass: out[n * M + m] = max (as double bits) of |x[n, q, m, j]| over q < Lq, j < inner, for x [N, Lq, M, inner]
+// (grad_out: inner = D; attn: inner = L * P).  A max is exact and the bit patterns of non-negative doubles order like
+// their values, so atomicMax on the bits is deterministic; NaN (sign cleared) and +inf land at or above the bits of
+// +inf, which marks the slice non-finite.  Block b covers slice b / chunks; its warps take every (chunks * 8)-th query
+// row, the lanes stride over the row's `inner` elements.
+__device__ __forceinline__ double ld1d(const float* p) { return (double)__ldg(p); }
+__device__ __forceinline__ double ld1d(const double* p) { return __ldg(p); }
+__device__ __forceinline__ double ld1d(const __half* p) { return (double)__half2float(__ldg(p)); }
+__device__ __forceinline__ double ld1d(const __nv_bfloat16* p) { return (double)__bfloat162float(__ldg(p)); }
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+msda_absmax_kernel(const T* __restrict__ x, unsigned long long* __restrict__ out, int M, int Lq, int inner,
+                   int chunks) {
+  const long long nm = blockIdx.x / chunks;
+  const long long n = nm / M, m = nm % M;
+  const int lane = threadIdx.x & 31;
+  unsigned long long mx = 0;
+  for (int q = (int)(blockIdx.x % chunks) * 8 + (threadIdx.x >> 5); q < Lq; q += chunks * 8) {
+    const T* row = x + ((n * Lq + q) * M + m) * inner;
+    for (int c = lane; c < inner; c += 32)
+      mx = max(mx, (unsigned long long)__double_as_longlong(fabs(ld1d(row + c))));
+  }
+  for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0 && mx) atomicMax(out + nm, mx);
+}
+
+__device__ __forceinline__ void st1d(float* p, double v) { *p = (float)v; }
+__device__ __forceinline__ void st1d(double* p, double v) { *p = v; }
+__device__ __forceinline__ void st1d(__half* p, double v) { *p = __double2half(v); }
+__device__ __forceinline__ void st1d(__nv_bfloat16* p, double v) { *p = __double2bfloat16(v); }
+
+// Finalize: grad_value[n, i, m, c] = sum * 2^-s of its (n, m) slice in Tout; NaN in a non-finite slice.  The sum goes to
+// double exactly while |sum| <= 2^53 and is then rounded once to Tout; a larger sum is rounded to double first (two
+// roundings, still a function of the sum alone).
+// One warp per pixel row (n, i) of M * D elements.
+template <typename Tout>
+__global__ void __launch_bounds__(256)
+msda_fixed_finalize_kernel(const MsdaFixedAcc acc, Tout* __restrict__ grad_value, int N, int S, int M, int D) {
+  const int lane = threadIdx.x & 31, MD = M * D;
+  const long long rows = (long long)N * S, warps = (long long)gridDim.x * 8;
+  for (long long r = blockIdx.x * 8LL + (threadIdx.x >> 5); r < rows; r += warps) {
+    const long long n = r / S;
+    for (int j = lane; j < MD; j += 32) {
+      const long long nm = n * M + j / D, i = r * MD + j;
+      double v;
+      if (acc.gmax[nm] >= MSDA_INF_BITS || acc.amax[nm] >= MSDA_INF_BITS) v = __longlong_as_double(MSDA_NAN_BITS);
+      else v = ldexp((double)(long long)acc.sum[i], -msda_fixed_shift(acc, nm));
+      st1d(grad_value + i, v);
     }
   }
 }
@@ -630,38 +804,100 @@ extern "C" int odise_msda_forward_f64(const double* value, const int64_t* spatia
   return (int)cudaGetLastError();
 }
 
+// Workspace of the deterministic backward entry points (odise_msda_det_workspace_bytes): the int64 sums [N, S, M, D],
+// then per (n, m) the max-|grad_out| and max-|attn| bits of MsdaFixedAcc.
+static long long det_ws_bytes(int N, int S, int M, int D) {
+  return (long long)sizeof(unsigned long long) * ((long long)N * S * M * D + 2LL * N * M);
+}
+
+static MsdaFixedAcc det_acc(void* ws, int N, int S, int M, int D, int Lq, int P) {
+  MsdaFixedAcc a;
+  a.sum = static_cast<unsigned long long*>(ws);
+  a.gmax = a.sum + (long long)N * S * M * D;
+  a.amax = a.gmax + (long long)N * M;
+  const long long K = (long long)Lq * P;
+  a.log2k = 0;
+  while ((1LL << a.log2k) < K) ++a.log2k;
+  return a;
+}
+
+template <typename T>
+static void launch_absmax(const T* x, unsigned long long* out, int N, int M, int Lq, int inner, cudaStream_t stream) {
+  const long long slices = (long long)N * M;
+  const long long most = (Lq + 7) / 8;                 // one query row per warp at least
+  long long chunks = (4LL * num_sms() * 8 + slices - 1) / slices;
+  if (chunks > most) chunks = most;
+  msda_absmax_kernel<T><<<(unsigned)(slices * chunks), 256, 0, stream>>>(x, out, M, Lq, inner, (int)chunks);
+}
+
+// Zero the workspace and run the exponent pre-pass (attn == nullptr: the fused paths, A = 1).
+template <typename T>
+static int det_begin(const MsdaFixedAcc& a, void* ws, const T* grad_out, const T* attn, int N, int S, int M, int D,
+                     int L, int Lq, int P, cudaStream_t stream) {
+  cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)det_ws_bytes(N, S, M, D), stream);
+  if (e != cudaSuccess) return (int)e;
+  launch_absmax<T>(grad_out, a.gmax, N, M, Lq, D, stream);
+  if (attn) launch_absmax<T>(attn, const_cast<unsigned long long*>(a.amax), N, M, Lq, L * P, stream);
+  return 0;
+}
+
+template <typename Tout>
+static void det_finish(const MsdaFixedAcc& a, Tout* grad_value, int N, int S, int M, int D, cudaStream_t stream) {
+  long long blocks = ((long long)N * S + 7) / 8;
+  if (blocks > num_sms() * 16LL) blocks = num_sms() * 16LL;
+  msda_fixed_finalize_kernel<Tout><<<(unsigned)blocks, 256, 0, stream>>>(a, grad_value, N, S, M, D);
+}
+
+// det = true: the deterministic twin (fixed-point grad_value through `ws`), otherwise the atomic default.
 template <typename T>
 static int msda_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start, const T* loc,
                          const T* attn, const T* grad_out, T* grad_value, T* grad_loc, T* grad_attn, int N, int S, int M,
-                         int D, int L, int Lq, int P, void* stream_v) {
+                         int D, int L, int Lq, int P, bool det, void* ws, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value || !spatial_shapes || !level_start || !loc || !attn || !grad_out || !grad_value || !grad_loc || !grad_attn)
     return ODISE_ERR_ARG;
+  if (det && !ws) return ODISE_ERR_WORKSPACE;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
   const long long pairs = (long long)N * Lq * M;
   if ((pairs + 7) / 8 > 0x7fffffffLL) return ODISE_ERR_ARG;   // grid of the generic path
   MsdaLevels lv{spatial_shapes, level_start};
-  // the reference returns at::zeros_like(value) plus the scattered contributions
-  cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(T) * (size_t)N * S * M * D, stream);
-  if (e != cudaSuccess) return (int)e;
-  bool d32 = false;
-  if constexpr (std::is_same<T, float>::value) {
-    if (d32_ok(S, M, D, L, P)) {
-      // 48 B of shared memory per (pair, sample): at most 32 x 32 x 48 = 48 KB, the default dynamic limit
-      const size_t smem = (size_t)MSDA_PAIRS * L * P * (sizeof(int4) + 2 * sizeof(float4));
-      const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
-      msda_d32_backward_kernel<0, float><<<blocks, 256, smem, stream>>>(value, lv, loc, attn, grad_out, grad_value,
-                                                                        grad_loc, grad_attn, N, S, M, L, Lq, P, nullptr,
-                                                                        1);
-      d32 = true;
+  MsdaFixedAcc fx{};
+  if (det) {
+    fx = det_acc(ws, N, S, M, D, Lq, P);
+    const int rc = det_begin<T>(fx, ws, grad_out, attn, N, S, M, D, L, Lq, P, stream);
+    if (rc) return rc;
+  } else {
+    // the reference returns at::zeros_like(value) plus the scattered contributions
+    cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(T) * (size_t)N * S * M * D, stream);
+    if (e != cudaSuccess) return (int)e;
+  }
+  auto run = [&](auto acc) {
+    using Acc = decltype(acc);
+    bool d32 = false;
+    if constexpr (std::is_same<T, float>::value) {
+      if (d32_ok(S, M, D, L, P)) {
+        // 48 B of shared memory per (pair, sample): at most 32 x 32 x 48 = 48 KB, the default dynamic limit
+        const size_t smem = (size_t)MSDA_PAIRS * L * P * (sizeof(int4) + 2 * sizeof(float4));
+        const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
+        msda_d32_backward_kernel<0, float, Acc><<<blocks, 256, smem, stream>>>(
+            value, lv, loc, attn, grad_out, grad_value, grad_loc, grad_attn, N, S, M, L, Lq, P, nullptr, 1, acc);
+        d32 = true;
+      }
     }
+    if (!d32) {
+      const long long blocks = (pairs + 7) / 8;       // one warp per (query, head) pair
+      msda_backward_warp_kernel<T, Acc><<<(unsigned)blocks, 256, 0, stream>>>(
+          value, lv, loc, attn, grad_out, grad_value, grad_loc, grad_attn, N, S, M, D, L, Lq, P, acc);
+    }
+  };
+  if (det) {
+    run(fx);
+    det_finish<T>(fx, grad_value, N, S, M, D, stream);
+    count_launch(4);
+  } else {
+    run(MsdaAtomicAcc{});
+    count_launch(1);
   }
-  if (!d32) {
-    const long long blocks = (pairs + 7) / 8;       // one warp per (query, head) pair
-    msda_backward_warp_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(value, lv, loc, attn, grad_out, grad_value,
-                                                                       grad_loc, grad_attn, N, S, M, D, L, Lq, P);
-  }
-  count_launch(1);
   return (int)cudaGetLastError();
 }
 
@@ -670,7 +906,7 @@ extern "C" int odise_msda_backward_f32(const float* value, const int64_t* spatia
                                        float* grad_loc, float* grad_attn, int N, int S, int M, int D, int L, int Lq,
                                        int P, void* stream) {
   return msda_backward<float>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,
-                              N, S, M, D, L, Lq, P, stream);
+                              N, S, M, D, L, Lq, P, false, nullptr, stream);
 }
 
 extern "C" int odise_msda_backward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -678,7 +914,30 @@ extern "C" int odise_msda_backward_f64(const double* value, const int64_t* spati
                                        double* grad_value, double* grad_loc, double* grad_attn, int N, int S, int M,
                                        int D, int L, int Lq, int P, void* stream) {
   return msda_backward<double>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc,
-                               grad_attn, N, S, M, D, L, Lq, P, stream);
+                               grad_attn, N, S, M, D, L, Lq, P, false, nullptr, stream);
+}
+
+extern "C" long long odise_msda_det_workspace_bytes(int N, int S, int M, int D) {
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0) return 0;
+  return det_ws_bytes(N, S, M, D);
+}
+
+extern "C" int odise_msda_backward_det_f32(const float* value, const int64_t* spatial_shapes,
+                                           const int64_t* level_start, const float* loc, const float* attn,
+                                           const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
+                                           int N, int S, int M, int D, int L, int Lq, int P, void* workspace,
+                                           void* stream) {
+  return msda_backward<float>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,
+                              N, S, M, D, L, Lq, P, true, workspace, stream);
+}
+
+extern "C" int odise_msda_backward_det_f64(const double* value, const int64_t* spatial_shapes,
+                                           const int64_t* level_start, const double* loc, const double* attn,
+                                           const double* grad_out, double* grad_value, double* grad_loc,
+                                           double* grad_attn, int N, int S, int M, int D, int L, int Lq, int P,
+                                           void* workspace, void* stream) {
+  return msda_backward<double>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc,
+                               grad_attn, N, S, M, D, L, Lq, P, true, workspace, stream);
 }
 
 extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
@@ -734,33 +993,49 @@ extern "C" int odise_msda_fused_bf16(const void* value, const int64_t* spatial_s
                                       stream);
 }
 
-// The fused backward for storage type T; grad_value is an fp32 buffer for every T.
+// The fused backward for storage type T.  Default (det = false): grad_value is an fp32 buffer for every T, accumulated
+// with fp32 atomics.  det = true: grad_value is in T, written by the fixed-point finalize pass through `ws`.
 template <typename T>
 static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                               const float* ref, const T* offs, const T* logits, const T* grad_out, float* grad_value,
+                               const float* ref, const T* offs, const T* logits, const T* grad_out, void* grad_value,
                                T* grad_offs, T* grad_logits, int N, int S, int M, int D, int L, int Lq, int P,
-                               void* stream_v) {
+                               bool det, void* ws, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value || !spatial_shapes || !level_start || !ref || !offs || !logits || !grad_out || !grad_value || !grad_offs ||
       !grad_logits)
     return ODISE_ERR_ARG;
+  if (det && !ws) return ODISE_ERR_WORKSPACE;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
   if (!d32_ok(S, M, D, L, P)) return ODISE_ERR_UNSUPPORTED;
   const long long pairs = (long long)N * Lq * M;
   const long long blocks = (pairs + MSDA_PAIRS - 1) / MSDA_PAIRS;
   if (blocks > 0x7fffffffLL) return ODISE_ERR_ARG;
   MsdaLevels lv{spatial_shapes, level_start};
-  cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(float) * (size_t)N * S * M * D, stream);
-  if (e != cudaSuccess) return (int)e;
+  MsdaFixedAcc fx{};
+  if (det) {
+    fx = det_acc(ws, N, S, M, D, Lq, P);
+    const int rc = det_begin<T>(fx, ws, grad_out, nullptr, N, S, M, D, L, Lq, P, stream);
+    if (rc) return rc;
+  } else {
+    cudaError_t e = cudaMemsetAsync(grad_value, 0, sizeof(float) * (size_t)N * S * M * D, stream);
+    if (e != cudaSuccess) return (int)e;
+  }
   const int LP = L * P;
   int SL = 1;
   while (SL < LP) SL <<= 1;
   // 48 B of shared memory per (pair, sample), as in the non-fused backward: at most 48 KB at L*P = 32
   const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + 2 * sizeof(float4));
-  msda_d32_backward_kernel<1, T><<<(unsigned)blocks, 256, smem, stream>>>(value, lv, offs, logits, grad_out, grad_value,
-                                                                          grad_offs, grad_logits, N, S, M, L, Lq, P,
-                                                                          ref, SL);
-  count_launch(1);
+  if (det) {
+    msda_d32_backward_kernel<1, T, MsdaFixedAcc><<<(unsigned)blocks, 256, smem, stream>>>(
+        value, lv, offs, logits, grad_out, nullptr, grad_offs, grad_logits, N, S, M, L, Lq, P, ref, SL, fx);
+    det_finish<T>(fx, static_cast<T*>(grad_value), N, S, M, D, stream);
+    count_launch(3);
+  } else {
+    msda_d32_backward_kernel<1, T><<<(unsigned)blocks, 256, smem, stream>>>(
+        value, lv, offs, logits, grad_out, static_cast<float*>(grad_value), grad_offs, grad_logits, N, S, M, L, Lq, P,
+        ref, SL, MsdaAtomicAcc{});
+    count_launch(1);
+  }
   return (int)cudaGetLastError();
 }
 
@@ -770,7 +1045,7 @@ extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* 
                                              float* grad_offs, float* grad_logits, int N, int S, int M, int D, int L,
                                              int Lq, int P, void* stream) {
   return msda_fused_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, stream);
+                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
 }
 
 extern "C" int odise_msda_fused_backward_f16(const void* value, const int64_t* spatial_shapes,
@@ -782,7 +1057,7 @@ extern "C" int odise_msda_fused_backward_f16(const void* value, const int64_t* s
   return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
                                 static_cast<const T*>(offs), static_cast<const T*>(logits),
                                 static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, stream);
+                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, false, nullptr, stream);
 }
 
 extern "C" int odise_msda_fused_backward_bf16(const void* value, const int64_t* spatial_shapes,
@@ -794,5 +1069,47 @@ extern "C" int odise_msda_fused_backward_bf16(const void* value, const int64_t* 
   return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
                                 static_cast<const T*>(offs), static_cast<const T*>(logits),
                                 static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, stream);
+                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, false, nullptr, stream);
+}
+
+// Deterministic twins of the fused backward: arguments of the default entry points plus the workspace; grad_value in
+// the storage type.
+extern "C" int odise_msda_fused_backward_det_f32(const float* value, const int64_t* spatial_shapes,
+                                                 const int64_t* level_start, const float* ref, const float* offs,
+                                                 const float* logits, const float* grad_out, float* grad_value,
+                                                 float* grad_offs, float* grad_logits, int N, int S, int M, int D,
+                                                 int L, int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
+}
+
+template <typename T>
+static int msda_fused_backward_det_16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                      void* grad_value, void* grad_offs, void* grad_logits, int N, int S, int M, int D,
+                                      int L, int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
+                                static_cast<const T*>(offs), static_cast<const T*>(logits),
+                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
+                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, true, workspace, stream);
+}
+
+extern "C" int odise_msda_fused_backward_det_f16(const void* value, const int64_t* spatial_shapes,
+                                                 const int64_t* level_start, const float* ref, const void* offs,
+                                                 const void* logits, const void* grad_out, void* grad_value,
+                                                 void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                                 int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_backward_det_16<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
+                                            grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, workspace,
+                                            stream);
+}
+
+extern "C" int odise_msda_fused_backward_det_bf16(const void* value, const int64_t* spatial_shapes,
+                                                  const int64_t* level_start, const float* ref, const void* offs,
+                                                  const void* logits, const void* grad_out, void* grad_value,
+                                                  void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                                  int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_backward_det_16<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
+                                                   grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, workspace,
+                                                   stream);
 }

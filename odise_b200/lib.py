@@ -57,6 +57,12 @@ _SIGS = {
     "odise_msda_fused_bf16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
     "odise_msda_fused_backward_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
     "odise_msda_fused_backward_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_det_workspace_bytes": [c_int] * 4,           # returns long long (set in load())
+    "odise_msda_backward_det_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_backward_det_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -165,6 +171,7 @@ def load():
         fn = getattr(lib, name)
         fn.argtypes = args
         fn.restype = c_int
+    lib.odise_msda_det_workspace_bytes.restype = c_longlong
     _lib = lib
     return lib
 
@@ -506,11 +513,19 @@ def msda_forward_f64(value, spatial_shapes, level_start_index, sampling_location
     return out
 
 
-def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=128):
+def _msda_det_workspace(N, S, M, D, device):
+    """workspace of the deterministic backward entry points (odise_msda_det_workspace_bytes), from torch's allocator"""
+    return torch.empty(int(load().odise_msda_det_workspace_bytes(N, S, M, D)), dtype=torch.uint8, device=device)
+
+
+def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=128,
+                  *, deterministic=False):
     """Drop-in for MSDA.ms_deform_attn_backward (reference ops/src/vision.cpp:20): same arguments, returns
     [grad_value, grad_sampling_loc, grad_attn_weight] shaped like value / sampling_loc / attn_weight.  float32 or
     float64 (all tensors of one dtype); RuntimeError on CPU, non-contiguous or mixed-dtype input and on a batch that
-    min(batch, im2col_step) does not divide.  The whole batch is one launch (im2col_step only checked)."""
+    min(batch, im2col_step) does not divide.  The whole batch is one launch (im2col_step only checked).
+    deterministic=True runs odise_msda_backward_det_f32 / _f64: grad_value summed in int64 fixed point, so its bits depend
+    on the inputs only (include/odise_b200.h states the error bound); the other two results are the same bits."""
     dtype = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
                           (grad_output, "grad_output")), im2col_step)
     N, S, M, D = value.shape
@@ -522,9 +537,16 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     grad_value = torch.empty_like(value)
     grad_loc = torch.empty_like(sampling_loc)
     grad_attn = torch.empty_like(attn_weight)
-    fn = "odise_msda_backward_f32" if dtype == torch.float32 else "odise_msda_backward_f64"
-    _check(getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output),
-                               _ptr(grad_value), _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P, _stream()), fn)
+    sfx = "f32" if dtype == torch.float32 else "f64"
+    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output), _ptr(grad_value),
+            _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P)
+    if deterministic:
+        ws = _msda_det_workspace(N, S, M, D, value.device)
+        fn = "odise_msda_backward_det_" + sfx
+        _check(getattr(load(), fn)(*args, _ptr(ws), _stream()), fn)
+    else:
+        fn = "odise_msda_backward_" + sfx
+        _check(getattr(load(), fn)(*args, _stream()), fn)
     return [grad_value, grad_loc, grad_attn]
 
 
@@ -576,22 +598,28 @@ def msda_fused_forward(value, spatial_shapes, level_start_index, reference_point
     return out
 
 
-def msda_fused_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output):
+def msda_fused_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output, *,
+                        deterministic=False):
     """Backward of msda_fused_forward (odise_msda_fused_backward_f32) -> (grad_value, grad_offsets, grad_logits) shaped
     like value / offsets / logits.  D = 32 and L*P <= 32 only; RuntimeError otherwise and on the input errors of
-    msda_fused_forward.  grad_offsets and grad_logits are bit-deterministic."""
+    msda_fused_forward.  grad_offsets and grad_logits are bit-deterministic; deterministic=True
+    (odise_msda_fused_backward_det_f32) makes grad_value so too."""
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output)
     grad_value = torch.empty_like(value)
     grad_offs = torch.empty_like(offsets)
     grad_logits = torch.empty_like(logits)
-    rc = load().odise_msda_fused_backward_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
-                                              _ptr(logits), _ptr(grad_output), _ptr(grad_value), _ptr(grad_offs),
-                                              _ptr(grad_logits), N, S, M, D, L, Lq, P, _stream())
+    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
+            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
+    if deterministic:
+        fn = "odise_msda_fused_backward_det_f32"
+        rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
+    else:
+        fn = "odise_msda_fused_backward_f32"
+        rc = getattr(load(), fn)(*args, _stream())
     if rc == ODISE_ERR_UNSUPPORTED:
-        raise OdiseError(f"odise_msda_fused_backward_f32: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and "
-                         "S*M*D < 2^31 only)")
-    _check(rc, "odise_msda_fused_backward_f32")
+        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
+    _check(rc, fn)
     return grad_value, grad_offs, grad_logits
 
 
@@ -627,21 +655,28 @@ def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference
     return out
 
 
-def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output):
+def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
+                              *, deterministic=False):
     """Backward of msda_fused_forward_16bit (odise_msda_fused_backward_f16 / _bf16) -> (grad_value, grad_offsets,
     grad_logits), each in the value's dtype.  grad_value is accumulated in a float32 buffer and rounded once here;
     grad_offsets and grad_logits are rounded once in the kernel and are bit-deterministic.  grad_output has the value's
-    dtype.  Errors as msda_fused_forward_16bit."""
+    dtype.  Errors as msda_fused_forward_16bit.  deterministic=True (odise_msda_fused_backward_det_f16 / _bf16) sums
+    grad_value in int64 fixed point and the kernels write it in the value's dtype: its bits depend on the inputs only."""
     sfx = _msda_16bit_suffix(value)
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output, dtype=value.dtype)
-    grad_value = torch.empty(value.shape, dtype=torch.float32, device=value.device)
+    grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
     grad_offs = torch.empty_like(offsets)
     grad_logits = torch.empty_like(logits)
+    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
+            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
+    if deterministic:
+        fn = "odise_msda_fused_backward_det_" + sfx
+        rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
+        _msda_16bit_rc(rc, fn, D, L, P)
+        return grad_value, grad_offs, grad_logits
     fn = "odise_msda_fused_backward_" + sfx
-    rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
-                             _ptr(grad_output), _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P,
-                             _stream())
+    rc = getattr(load(), fn)(*args, _stream())
     _msda_16bit_rc(rc, fn, D, L, P)
     return grad_value.to(value.dtype), grad_offs, grad_logits
 

@@ -10,7 +10,8 @@ MSDeformAttnFunction is the autograd Function of ops/functions/ms_deform_attn_fu
 MSDeformAttnFusedFunction differentiates the fused op (odise_msda_fused_f32 / odise_msda_fused_backward_f32: softmax and
 sampling locations computed inside the kernels; float16 and bfloat16 storage under autocast), and MSDeformAttn is the
 module of ops/modules/ms_deform_attn.py, which takes the fused op where it applies.  All of them run the library's sm_90a
-kernels; there is no CPU path."""
+kernels; there is no CPU path.  Under torch.use_deterministic_algorithms(True) every backward here returns a
+bit-reproducible grad_value (fixed-point sums, lib's deterministic=True); the other gradients are deterministic anyway."""
 import math
 import warnings
 
@@ -35,8 +36,10 @@ class MSDA:
     @staticmethod
     def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
                                 im2col_step):
+        """Under torch.use_deterministic_algorithms(True) (warn_only too) grad_value is summed in fixed point and is
+        bit-reproducible; otherwise float atomics, as in the reference."""
         return lib.msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
-                                 im2col_step)
+                                 im2col_step, deterministic=torch.are_deterministic_algorithms_enabled())
 
 
 class MSDeformAttnFunction(Function):
@@ -91,7 +94,7 @@ class MSDeformAttnFusedFunction(Function):
         bwd = lib.msda_fused_backward_16bit if value.dtype in _LOW else lib.msda_fused_backward
         grad_value, grad_offsets, grad_logits = bwd(
             value, spatial_shapes, level_start_index, reference_points, offsets, logits,
-            grad_output.to(value.dtype).contiguous())
+            grad_output.to(value.dtype).contiguous(), deterministic=torch.are_deterministic_algorithms_enabled())
         grad_ref = None
         if ctx.needs_input_grad[3]:
             go = grad_offsets.float()
