@@ -513,6 +513,16 @@ def msda_forward_f64(value, spatial_shapes, level_start_index, sampling_location
     return out
 
 
+def _msda_backward_shapes(value, sampling_loc, grad_output):
+    """(N, S, M, D, L, Lq, P) of msda_backward's layouts (value [N, S, M, D], sampling_loc [N, Lq, M, L, P, 2]); raises
+    unless grad_output has N * Lq * M * D elements."""
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = sampling_loc.shape
+    if grad_output.numel() != N * Lq * M * D:
+        raise OdiseError(f"grad_output: expected {N * Lq * M * D} elements, got {grad_output.numel()}")
+    return N, S, M, D, L, Lq, P
+
+
 def _msda_det_workspace(N, S, M, D, device):
     """workspace of the deterministic backward entry points (odise_msda_det_workspace_bytes), from torch's allocator"""
     return torch.empty(int(load().odise_msda_det_workspace_bytes(N, S, M, D)), dtype=torch.uint8, device=device)
@@ -528,10 +538,7 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     on the inputs only (include/odise_b200.h states the error bound); the other two results are the same bits."""
     dtype = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
                           (grad_output, "grad_output")), im2col_step)
-    N, S, M, D = value.shape
-    _, Lq, _, L, P, _ = sampling_loc.shape
-    if grad_output.numel() != N * Lq * M * D:
-        raise OdiseError(f"grad_output: expected {N * Lq * M * D} elements, got {grad_output.numel()}")
+    N, S, M, D, L, Lq, P = _msda_backward_shapes(value, sampling_loc, grad_output)
     ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
     ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
     grad_value = torch.empty_like(value)
@@ -551,6 +558,14 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
 
 
 ODISE_ERR_UNSUPPORTED = 10006
+
+
+def _msda_d32_only(fn, S, M, D, L, P):
+    """The shapes the fused backward and the 16-bit fused forward take (d32_ok in msda.cu; their entry points return
+    ODISE_ERR_UNSUPPORTED on any other): D = 32, L*P <= 32 and S*M*D < 2^31.  Raises before any launch, and needs no
+    library, so that the fake implementations of odise_b200.msda's ops refuse the same shapes."""
+    if not (D == 32 and L * P <= 32 and S * M * D < 2 ** 31):
+        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
 
 
 def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
@@ -606,19 +621,17 @@ def msda_fused_backward(value, spatial_shapes, level_start_index, reference_poin
     (odise_msda_fused_backward_det_f32) makes grad_value so too."""
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output)
+    fn = "odise_msda_fused_backward_det_f32" if deterministic else "odise_msda_fused_backward_f32"
+    _msda_d32_only(fn, S, M, D, L, P)
     grad_value = torch.empty_like(value)
     grad_offs = torch.empty_like(offsets)
     grad_logits = torch.empty_like(logits)
     args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
             _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
     if deterministic:
-        fn = "odise_msda_fused_backward_det_f32"
         rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
     else:
-        fn = "odise_msda_fused_backward_f32"
         rc = getattr(load(), fn)(*args, _stream())
-    if rc == ODISE_ERR_UNSUPPORTED:
-        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
     _check(rc, fn)
     return grad_value, grad_offs, grad_logits
 
@@ -633,12 +646,6 @@ def _msda_16bit_suffix(value):
     return _MSDA_16BIT[value.dtype]
 
 
-def _msda_16bit_rc(rc, fn, D, L, P):
-    if rc == ODISE_ERR_UNSUPPORTED:
-        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
-    _check(rc, fn)
-
-
 def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
     """msda_fused_forward with 16-bit storage (odise_msda_fused_f16 / _bf16, chosen by value.dtype): value, offsets and
     logits float16 or bfloat16 (one dtype), reference_points float32 -> out [N, Lq, M*D] in the value's dtype, one rounding
@@ -647,11 +654,12 @@ def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference
     sfx = _msda_16bit_suffix(value)
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, dtype=value.dtype)
-    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
     fn = "odise_msda_fused_" + sfx
+    _msda_d32_only(fn, S, M, D, L, P)
+    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
     rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
                              _ptr(out), N, S, M, D, L, Lq, P, _stream())
-    _msda_16bit_rc(rc, fn, D, L, P)
+    _check(rc, fn)
     return out
 
 
@@ -665,19 +673,19 @@ def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, referenc
     sfx = _msda_16bit_suffix(value)
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output, dtype=value.dtype)
+    fn = ("odise_msda_fused_backward_det_" if deterministic else "odise_msda_fused_backward_") + sfx
+    _msda_d32_only(fn, S, M, D, L, P)
     grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
     grad_offs = torch.empty_like(offsets)
     grad_logits = torch.empty_like(logits)
     args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
             _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
     if deterministic:
-        fn = "odise_msda_fused_backward_det_" + sfx
         rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
-        _msda_16bit_rc(rc, fn, D, L, P)
+        _check(rc, fn)
         return grad_value, grad_offs, grad_logits
-    fn = "odise_msda_fused_backward_" + sfx
     rc = getattr(load(), fn)(*args, _stream())
-    _msda_16bit_rc(rc, fn, D, L, P)
+    _check(rc, fn)
     return grad_value.to(value.dtype), grad_offs, grad_logits
 
 

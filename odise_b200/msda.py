@@ -11,7 +11,10 @@ MSDeformAttnFusedFunction differentiates the fused op (odise_msda_fused_f32 / od
 sampling locations computed inside the kernels; float16 and bfloat16 storage under autocast), and MSDeformAttn is the
 module of ops/modules/ms_deform_attn.py, which takes the fused op where it applies.  All of them run the library's sm_90a
 kernels; there is no CPU path.  Under torch.use_deterministic_algorithms(True) every backward here returns a
-bit-reproducible grad_value (fixed-point sums, lib's deterministic=True); the other gradients are deterministic anyway."""
+bit-reproducible grad_value (fixed-point sums, lib's deterministic=True); the other gradients are deterministic anyway.
+They reach the kernels through four torch custom ops (torch.ops.odise_b200.msda_forward, msda_backward,
+msda_fused_forward, msda_fused_backward) with fake implementations, so torch.compile (fullgraph=True included) and
+torch.export trace them without a graph break."""
 import math
 import warnings
 
@@ -24,22 +27,116 @@ from torch.autograd.function import once_differentiable
 from . import lib
 
 
+# The kernels as torch custom ops in namespace odise_b200, the one place where a traced graph (torch.compile,
+# torch.export) meets lib's ctypes calls, which Dynamo cannot trace.  The implementation is registered for every device,
+# so that a CPU tensor reaches lib's own check; the fake implementations give the results' shapes, dtypes and devices,
+# refuse what lib refuses for reasons visible without data (with lib's own validators) and never load the library.
+# torch.library.Library rather than torch.library.custom_op: its eager call goes straight to the dispatcher, without
+# custom_op's Python wrapper (DESIGN.md §3, "Under torch.compile").  There is no autograd formula on the ops: the Functions below are the
+# one autograd definition, and Dynamo traces them with the ops inside.
+_OPS = torch.library.Library("odise_b200", "DEF")
+_OPS.define("msda_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
+            "Tensor attn_weight, int im2col_step) -> Tensor")
+_OPS.define("msda_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
+            "Tensor attn_weight, Tensor grad_output, int im2col_step, bool deterministic) -> (Tensor, Tensor, Tensor)")
+_OPS.define("msda_fused_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
+            "Tensor reference_points, Tensor offsets, Tensor logits) -> Tensor")
+_OPS.define("msda_fused_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
+            "Tensor reference_points, Tensor offsets, Tensor logits, Tensor grad_output, bool deterministic) "
+            "-> (Tensor, Tensor, Tensor)")
+_LOW = (torch.float16, torch.bfloat16)
+
+
+# lib's functions are looked up at call time, so that a test that patches them sees every call
+def _msda_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
+    fwd = lib.msda_forward_f64 if value.dtype == torch.float64 else lib.msda_forward
+    return fwd(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step)
+
+
+def _msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step,
+                   deterministic):
+    return tuple(lib.msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
+                                   im2col_step, deterministic=deterministic))
+
+
+def _msda_fused_forward(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+    fwd = lib.msda_fused_forward_16bit if value.dtype in _LOW else lib.msda_fused_forward
+    return fwd(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+
+
+def _msda_fused_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
+                         deterministic):
+    bwd = lib.msda_fused_backward_16bit if value.dtype in _LOW else lib.msda_fused_backward
+    return bwd(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
+               deterministic=deterministic)
+
+
+for _name, _fn in (("msda_forward", _msda_forward), ("msda_backward", _msda_backward),
+                   ("msda_fused_forward", _msda_fused_forward), ("msda_fused_backward", _msda_fused_backward)):
+    _OPS.impl(_name, _fn, "CompositeExplicitAutograd")
+
+
+@torch.library.register_fake("odise_b200::msda_forward", lib=_OPS)
+def _msda_forward_fake(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
+    lib._msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight")), im2col_step)
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = sampling_loc.shape
+    return value.new_empty(N, Lq, M * D)
+
+
+@torch.library.register_fake("odise_b200::msda_backward", lib=_OPS)
+def _msda_backward_fake(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step,
+                        deterministic):
+    lib._msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
+                      (grad_output, "grad_output")), im2col_step)
+    lib._msda_backward_shapes(value, sampling_loc, grad_output)
+    return torch.empty_like(value), torch.empty_like(sampling_loc), torch.empty_like(attn_weight)
+
+
+def _msda_fused_fake_shapes(op, value, spatial_shapes, level_start_index, reference_points, offsets, logits,
+                            grad_output=None):
+    """lib's checks of the fused op `op` (forward when grad_output is None) for value's dtype -> (N, Lq, M, D)"""
+    low = value.dtype in _LOW
+    N, S, M, D, L, Lq, P, _, _ = lib._msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
+                                                        offsets, logits, grad_output,
+                                                        dtype=value.dtype if low else torch.float32)
+    if low or grad_output is not None:
+        lib._msda_d32_only(op, S, M, D, L, P)
+    return N, Lq, M, D
+
+
+@torch.library.register_fake("odise_b200::msda_fused_forward", lib=_OPS)
+def _msda_fused_forward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+    N, Lq, M, D = _msda_fused_fake_shapes("odise_b200::msda_fused_forward", value, spatial_shapes, level_start_index,
+                                          reference_points, offsets, logits)
+    return value.new_empty(N, Lq, M * D)
+
+
+@torch.library.register_fake("odise_b200::msda_fused_backward", lib=_OPS)
+def _msda_fused_backward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
+                              deterministic):
+    _msda_fused_fake_shapes("odise_b200::msda_fused_backward", value, spatial_shapes, level_start_index,
+                            reference_points, offsets, logits, grad_output)
+    return torch.empty_like(value), torch.empty_like(offsets), torch.empty_like(logits)
+
+
 class MSDA:
     """Stand-in for the pybind module: ms_deform_attn_forward / ms_deform_attn_backward (ops/src/vision.cpp:19-20)."""
 
     @staticmethod
     def ms_deform_attn_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
-        if value.dtype == torch.float64:
-            return lib.msda_forward_f64(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step)
-        return lib.msda_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step)
+        return torch.ops.odise_b200.msda_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight,
+                                                 im2col_step)
 
     @staticmethod
     def ms_deform_attn_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
                                 im2col_step):
         """Under torch.use_deterministic_algorithms(True) (warn_only too) grad_value is summed in fixed point and is
-        bit-reproducible; otherwise float atomics, as in the reference."""
-        return lib.msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output,
-                                 im2col_step, deterministic=torch.are_deterministic_algorithms_enabled())
+        bit-reproducible; otherwise float atomics, as in the reference.  Under torch.compile the switch is read when the
+        graph is traced (Dynamo guards on it: flipping it recompiles)."""
+        return list(torch.ops.odise_b200.msda_backward(value, spatial_shapes, level_start_index, sampling_loc,
+                                                       attn_weight, grad_output, im2col_step,
+                                                       torch.are_deterministic_algorithms_enabled()))
 
 
 class MSDeformAttnFunction(Function):
@@ -66,9 +163,6 @@ class MSDeformAttnFunction(Function):
         return grad_value, None, None, grad_sampling_loc, grad_attn_weight, None
 
 
-_LOW = (torch.float16, torch.bfloat16)
-
-
 class MSDeformAttnFusedFunction(Function):
     """Autograd through the fused op: forward odise_msda_fused_f32, backward odise_msda_fused_backward_f32, or their
     16-bit forms (odise_msda_fused_f16 / _bf16 and the backward) when value is float16 or bfloat16.
@@ -82,8 +176,8 @@ class MSDeformAttnFusedFunction(Function):
 
     @staticmethod
     def forward(ctx, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
-        fwd = lib.msda_fused_forward_16bit if value.dtype in _LOW else lib.msda_fused_forward
-        output = fwd(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
+        output = torch.ops.odise_b200.msda_fused_forward(value, spatial_shapes, level_start_index, reference_points,
+                                                         offsets, logits)
         ctx.save_for_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
         return output
 
@@ -91,10 +185,9 @@ class MSDeformAttnFusedFunction(Function):
     @once_differentiable
     def backward(ctx, grad_output):
         value, spatial_shapes, level_start_index, reference_points, offsets, logits = ctx.saved_tensors
-        bwd = lib.msda_fused_backward_16bit if value.dtype in _LOW else lib.msda_fused_backward
-        grad_value, grad_offsets, grad_logits = bwd(
+        grad_value, grad_offsets, grad_logits = torch.ops.odise_b200.msda_fused_backward(
             value, spatial_shapes, level_start_index, reference_points, offsets, logits,
-            grad_output.to(value.dtype).contiguous(), deterministic=torch.are_deterministic_algorithms_enabled())
+            grad_output.to(value.dtype).contiguous(), torch.are_deterministic_algorithms_enabled())
         grad_ref = None
         if ctx.needs_input_grad[3]:
             go = grad_offsets.float()
@@ -168,7 +261,8 @@ class MSDeformAttn(nn.Module):
             raise lib.OdiseError("MSDeformAttn: expected CUDA tensors (odise_b200 kernels only run on the GPU)")
         N, Lq, _ = query.shape
         _, S, _ = input_flatten.shape
-        assert (input_spatial_shapes[:, 0] * input_spatial_shapes[:, 1]).sum() == S
+        if not torch.compiler.is_compiling():  # reads the shapes on the host, which a traced graph cannot: skipped there
+            assert (input_spatial_shapes[:, 0] * input_spatial_shapes[:, 1]).sum() == S
         M, L, P = self.n_heads, self.n_levels, self.n_points
         D = self.d_model // M
         if reference_points.shape[-1] not in (2, 4):
