@@ -170,6 +170,55 @@ int odise_msda_fused_backward_det_bf16(const void* value, const int64_t* spatial
                                        void* grad_value, void* grad_offs, void* grad_logits,
                                        int N, int S, int M, int D, int L, int Lq, int P, void* workspace, void* stream);
 
+/* Box reference points (ms_deform_attn.py:110-112, the cross-attention of DETR-style decoders): the fused entry points
+ * above with ref [N, Lq, L, 4] = (cx, cy, w, h), float32 and 16-byte aligned (ODISE_ERR_ARG otherwise), and
+ *   loc = (cx + off.x / P * w * 0.5, cy + off.y / P * h * 0.5)
+ * computed in float32 with the roundings of the composed path's torch ops on the device (off / P as the product with the
+ * float32 reciprocal of P, then * w, * 0.5 and the sum), so both paths sample at the same float32 locations.  The
+ * backward writes the gradient of the raw offsets,
+ *   grad_offs = (W_l * aw * sum_c g_c * d bilinear_c / dw * w, H_l * aw * sum_c g_c * d bilinear_c / dh * h) * 0.5 / P,
+ * with no division by w or h: a degenerate box (w = 0 or h = 0) is valid and gives grad_offs = 0 along that axis.  The
+ * gradient of ref is not computed (it cannot be recovered from grad_offs without dividing by w and h).  Argument lists,
+ * storage types, grad_value buffers, workspace and determinism are those of the 2-column twins; the f32 forward takes no
+ * out_hi / out_lo.  Every box entry point runs the D = 32 kernels only: D = 32, L*P <= 32 and S*M*D < 2^31, in both
+ * directions and in float32 too (ODISE_ERR_UNSUPPORTED otherwise).  No host synchronisation and no allocation. */
+int odise_msda_fused_box_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                             const float* ref, const float* offs, const float* logits, float* out,
+                             int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                             const float* ref, const void* offs, const void* logits, void* out,
+                             int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                              const float* ref, const void* offs, const void* logits, void* out,
+                              int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_backward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref, const float* offs, const float* logits, const float* grad_out,
+                                      float* grad_value, float* grad_offs, float* grad_logits,
+                                      int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_backward_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                      const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                      float* grad_value, void* grad_offs, void* grad_logits,
+                                      int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_backward_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                       const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                       float* grad_value, void* grad_offs, void* grad_logits,
+                                       int N, int S, int M, int D, int L, int Lq, int P, void* stream);
+int odise_msda_fused_box_backward_det_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                          const float* ref, const float* offs, const float* logits,
+                                          const float* grad_out, float* grad_value, float* grad_offs,
+                                          float* grad_logits, int N, int S, int M, int D, int L, int Lq, int P,
+                                          void* workspace, void* stream);
+int odise_msda_fused_box_backward_det_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                          const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                          void* grad_value, void* grad_offs, void* grad_logits,
+                                          int N, int S, int M, int D, int L, int Lq, int P, void* workspace,
+                                          void* stream);
+int odise_msda_fused_box_backward_det_bf16(const void* value, const int64_t* spatial_shapes,
+                                           const int64_t* level_start, const float* ref, const void* offs,
+                                           const void* logits, const void* grad_out, void* grad_value,
+                                           void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                           int Lq, int P, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * wgmma GEMM / implicit-GEMM 3x3 convolution:  out[z][m][n] = epi(alpha * sum_k A[z][m][k] * B[z][n][k]).
  * Replaces F.conv2d / F.linear / torch.einsum call sites of the path (ldm ResBlock & attention linears via

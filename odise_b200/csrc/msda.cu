@@ -243,12 +243,15 @@ __device__ __forceinline__ MsdaCorners msda_corners(float lx, float ly, int H, i
 // differentiates exactly the bits its forward sampled with.  The softmax reduces over an aligned sub-warp of SL lanes
 // (slot = pair * SL + sample): every lane of the warp must make the call.  T is the storage type of the offsets and
 // logits (float, or 16-bit with FUSED = 1); they are converted to float as they are loaded, ref is always float.
+// RW is the width of a reference point: 2 = (x, y), 4 = a box (cx, cy, w, h) with loc = ref.xy + off / P * ref.wh * 0.5
+// (ms_deform_attn.py:110-112), computed with the roundings of the composed path's torch ops on the device: `off / P` by
+// a CUDA tensor is a product with the fp32 reciprocal of P, then the product with w, * 0.5 (exact) and the sum.
 struct MsdaSlot {
   float lx, ly, aw;
   int H, W, start;
 };
 
-template <int FUSED, typename T>
+template <int FUSED, typename T, int RW = 2>
 __device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const T* __restrict__ loc_or_off,
                                               const T* __restrict__ attn_or_logit, const float* __restrict__ ref,
                                               long long pair, int s, bool live, int M, int L, int P, int SL) {
@@ -264,7 +267,12 @@ __device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const T* __r
     const float2 xy = ld2(loc_or_off + (pair * LP + s) * 2);
     r.aw = ld1(attn_or_logit + pair * LP + s);
     r.lx = xy.x; r.ly = xy.y;
-    if (FUSED) {
+    if constexpr (FUSED && RW == 4) {
+      const float4 rp = __ldg(reinterpret_cast<const float4*>(ref + (pair / M * L + l) * 4));
+      const float inv_p = 1.f / (float)P;
+      r.lx = rp.x + xy.x * inv_p * rp.z * 0.5f;
+      r.ly = rp.y + xy.y * inv_p * rp.w * 0.5f;
+    } else if (FUSED) {
       const long long nq = pair / M;
       const float2 rp = __ldg(reinterpret_cast<const float2*>(ref + (nq * L + l) * 2));
       r.lx = rp.x + xy.x / (float)r.W;        // ms_deform_attn.py:104-107
@@ -284,7 +292,8 @@ __device__ __forceinline__ MsdaSlot msda_slot(const MsdaLevels& lv, const T* __r
 
 // T: storage type of value, loc_or_off, attn_or_logit and out.  float for both FUSED; __half / __nv_bfloat16 with
 // FUSED = 1 (odise_msda_fused_f16 / _bf16: a lane's 4 channels are one 64-bit load per corner, out_hi / out_lo unused).
-template <int FUSED, typename T>
+// RW: reference-point width of msda_slot (4: the odise_msda_fused_box_* entry points); only phase 1 differs.
+template <int FUSED, typename T, int RW = 2>
 __global__ void __launch_bounds__(256)
 msda_d32_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc_or_off,
                 const T* __restrict__ attn_or_logit, const float* __restrict__ ref, T* __restrict__ out,
@@ -303,7 +312,7 @@ msda_d32_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __res
     const int pl = slot / SL, s = slot - pl * SL;
     const long long pair = pair0 + pl;
     const bool live = (s < LP) && (pair < pairs);
-    const MsdaSlot sl = msda_slot<FUSED, T>(lv, loc_or_off, attn_or_logit, ref, pair, s, live, M, L, P, SL);
+    const MsdaSlot sl = msda_slot<FUSED, T, RW>(lv, loc_or_off, attn_or_logit, ref, pair, s, live, M, L, P, SL);
     if (live) {
       const float aw = sl.aw;
       const MsdaCorners cn = msda_corners(sl.lx, sl.ly, sl.H, sl.W, sl.start, pix);
@@ -344,7 +353,7 @@ static bool d32_ok(int S, int M, int D, int L, int P) {
   return D == 32 && L * P <= 32 && (long long)S * M * D < (1LL << 31);
 }
 
-template <int FUSED, typename T>
+template <int FUSED, typename T, int RW = 2>
 static void launch_d32(const T* value, const MsdaLevels& lv, const T* a, const T* b, const float* ref,
                        T* out, __nv_bfloat16* hi, __nv_bfloat16* lo, int N, int S, int M, int L, int Lq, int P,
                        cudaStream_t stream) {
@@ -354,7 +363,8 @@ static void launch_d32(const T* value, const MsdaLevels& lv, const T* a, const T
   const long long pairs = (long long)N * Lq * M;
   const int blocks = (int)((pairs + MSDA_PAIRS - 1) / MSDA_PAIRS);
   const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + sizeof(float4));
-  msda_d32_kernel<FUSED, T><<<blocks, 256, smem, stream>>>(value, lv, a, b, ref, out, hi, lo, N, S, M, L, Lq, P, SL);
+  msda_d32_kernel<FUSED, T, RW><<<blocks, 256, smem, stream>>>(value, lv, a, b, ref, out, hi, lo, N, S, M, L, Lq, P,
+                                                               SL);
 }
 
 static bool vec_ok(int D) { return D % 4 == 0 && D <= 128 && (32 % (D / 4) == 0); }
@@ -469,7 +479,13 @@ constexpr unsigned long long MSDA_INF_BITS = 0x7ff0000000000000ull;
 // integer reductions into acc.sum instead of one 128-bit float reduction.  For them lane j of a pair holds a second,
 // interleaved copy of grad_out (channels j, j + 8, j + 16, j + 24), so that each reduction instruction of the pair's 8
 // lanes covers 64 contiguous bytes; the contributions are the same products, summed by other lanes.
-template <int FUSED, typename T, typename Acc = MsdaAtomicAcc>
+//
+// RW = 4 (FUSED = 1, the odise_msda_fused_box_backward_* entry points): box reference points, phase 1 as in the forward.
+// d loc / d off = (w, h) * 0.5 / P does not cancel the W and H of grad_loc, so the storing lane writes
+// grad_off = (W * aw * sw * w, H * aw * sh * h) * 0.5 / P, reading (w, h) of its (query, level) from global memory (an L1
+// broadcast; the 48 B shared record per slot is full at L*P = 32).  Nothing is divided by w or h: a degenerate box
+// (w = 0 or h = 0) gives grad_off = 0 along that axis.
+template <int FUSED, typename T, typename Acc = MsdaAtomicAcc, int RW = 2>
 __global__ void __launch_bounds__(256)
 msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const T* __restrict__ loc,
                          const T* __restrict__ attn, const T* __restrict__ grad_out,
@@ -491,7 +507,7 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
       const int pl = slot / SL, s = slot - pl * SL;
       const long long pair = pair0 + pl;
       const bool live = (s < LP) && (pair < pairs);
-      const MsdaSlot sl = msda_slot<1, T>(lv, loc, attn, ref, pair, s, live, M, L, P, SL);
+      const MsdaSlot sl = msda_slot<1, T, RW>(lv, loc, attn, ref, pair, s, live, M, L, P, SL);
       if (s < LP) {
         int4 o4 = make_int4(0, 0, 0, 0);
         float4 w4 = make_float4(0.f, 0.f, 0.f, 0.f), f4 = w4;
@@ -600,7 +616,13 @@ msda_d32_backward_kernel(const T* __restrict__ value, const MsdaLevels lv, const
       if (FUSED) {
         __syncwarp();                                 // all lanes of the pair have read pf[s]: its lh is dead
         if (live && c == 0) {
-          st2(grad_loc + 2 * (pair * LP + s), make_float2(aw * sw, aw * sh));
+          if constexpr (RW == 4) {
+            const float2 wh = __ldg(reinterpret_cast<const float2*>(ref + (pair / M * L + l) * 4 + 2));
+            st2(grad_loc + 2 * (pair * LP + s),
+                make_float2(Wf * aw * sw * wh.x * 0.5f / (float)P, Hf * aw * sh * wh.y * 0.5f / (float)P));
+          } else {
+            st2(grad_loc + 2 * (pair * LP + s), make_float2(aw * sw, aw * sh));
+          }
           pf[s].x = sv;
         }
         dot = fmaf(aw, sv, dot);
@@ -963,19 +985,25 @@ extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_s
   return (int)cudaGetLastError();
 }
 
-// The fused forward in a 16-bit storage type T (odise_msda_fused_f16 / _bf16): D = 32 kernel only, no planes.
-template <typename T>
+// a box reference point [N, Lq, L, 4] is one 16-byte load
+static bool ref_ok(const float* ref, int RW) { return RW == 2 || reinterpret_cast<uintptr_t>(ref) % 16 == 0; }
+
+// The fused forward on the D = 32 kernel only, no planes: a 16-bit storage type T (odise_msda_fused_f16 / _bf16), and
+// with RW = 4 the box forms for every T (odise_msda_fused_box_f32 / _f16 / _bf16).
+template <typename T, int RW = 2>
 static int msda_fused_16(const void* value_v, const int64_t* spatial_shapes, const int64_t* level_start,
                          const float* ref, const void* offs_v, const void* logits_v, void* out_v, int N, int S, int M,
                          int D, int L, int Lq, int P, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value_v || !spatial_shapes || !level_start || !ref || !offs_v || !logits_v || !out_v) return ODISE_ERR_ARG;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  if (!ref_ok(ref, RW)) return ODISE_ERR_ARG;
   if (!d32_ok(S, M, D, L, P)) return ODISE_ERR_UNSUPPORTED;
   if (((long long)N * Lq * M + MSDA_PAIRS - 1) / MSDA_PAIRS > 0x7fffffffLL) return ODISE_ERR_ARG;
   MsdaLevels lv{spatial_shapes, level_start};
-  launch_d32<1, T>(static_cast<const T*>(value_v), lv, static_cast<const T*>(offs_v), static_cast<const T*>(logits_v),
-                   ref, static_cast<T*>(out_v), nullptr, nullptr, N, S, M, L, Lq, P, stream);
+  launch_d32<1, T, RW>(static_cast<const T*>(value_v), lv, static_cast<const T*>(offs_v),
+                       static_cast<const T*>(logits_v), ref, static_cast<T*>(out_v), nullptr, nullptr, N, S, M, L, Lq,
+                       P, stream);
   count_launch(1);
   return (int)cudaGetLastError();
 }
@@ -994,8 +1022,9 @@ extern "C" int odise_msda_fused_bf16(const void* value, const int64_t* spatial_s
 }
 
 // The fused backward for storage type T.  Default (det = false): grad_value is an fp32 buffer for every T, accumulated
-// with fp32 atomics.  det = true: grad_value is in T, written by the fixed-point finalize pass through `ws`.
-template <typename T>
+// with fp32 atomics.  det = true: grad_value is in T, written by the fixed-point finalize pass through `ws`.  RW = 4: box
+// reference points (odise_msda_fused_box_backward_*).
+template <typename T, int RW = 2>
 static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,
                                const float* ref, const T* offs, const T* logits, const T* grad_out, void* grad_value,
                                T* grad_offs, T* grad_logits, int N, int S, int M, int D, int L, int Lq, int P,
@@ -1006,6 +1035,7 @@ static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, co
     return ODISE_ERR_ARG;
   if (det && !ws) return ODISE_ERR_WORKSPACE;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
+  if (!ref_ok(ref, RW)) return ODISE_ERR_ARG;
   if (!d32_ok(S, M, D, L, P)) return ODISE_ERR_UNSUPPORTED;
   const long long pairs = (long long)N * Lq * M;
   const long long blocks = (pairs + MSDA_PAIRS - 1) / MSDA_PAIRS;
@@ -1026,12 +1056,12 @@ static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, co
   // 48 B of shared memory per (pair, sample), as in the non-fused backward: at most 48 KB at L*P = 32
   const size_t smem = (size_t)MSDA_PAIRS * LP * (sizeof(int4) + 2 * sizeof(float4));
   if (det) {
-    msda_d32_backward_kernel<1, T, MsdaFixedAcc><<<(unsigned)blocks, 256, smem, stream>>>(
+    msda_d32_backward_kernel<1, T, MsdaFixedAcc, RW><<<(unsigned)blocks, 256, smem, stream>>>(
         value, lv, offs, logits, grad_out, nullptr, grad_offs, grad_logits, N, S, M, L, Lq, P, ref, SL, fx);
     det_finish<T>(fx, static_cast<T*>(grad_value), N, S, M, D, stream);
     count_launch(3);
   } else {
-    msda_d32_backward_kernel<1, T><<<(unsigned)blocks, 256, smem, stream>>>(
+    msda_d32_backward_kernel<1, T, MsdaAtomicAcc, RW><<<(unsigned)blocks, 256, smem, stream>>>(
         value, lv, offs, logits, grad_out, static_cast<float*>(grad_value), grad_offs, grad_logits, N, S, M, L, Lq, P,
         ref, SL, MsdaAtomicAcc{});
     count_launch(1);
@@ -1112,4 +1142,94 @@ extern "C" int odise_msda_fused_backward_det_bf16(const void* value, const int64
   return msda_fused_backward_det_16<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
                                                    grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, workspace,
                                                    stream);
+}
+
+// Box reference points [N, Lq, L, 4] (cx, cy, w, h): the fused entry points above with RW = 4, on the D = 32 kernels in
+// every storage type (include/odise_b200.h states the formulas).
+extern "C" int odise_msda_fused_box_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                        const float* ref, const float* offs, const float* logits, float* out, int N,
+                                        int S, int M, int D, int L, int Lq, int P, void* stream) {
+  return msda_fused_16<float, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
+                                 stream);
+}
+
+extern "C" int odise_msda_fused_box_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                        const float* ref, const void* offs, const void* logits, void* out, int N, int S,
+                                        int M, int D, int L, int Lq, int P, void* stream) {
+  return msda_fused_16<__half, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
+                                  stream);
+}
+
+extern "C" int odise_msda_fused_box_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                         const float* ref, const void* offs, const void* logits, void* out, int N,
+                                         int S, int M, int D, int L, int Lq, int P, void* stream) {
+  return msda_fused_16<__nv_bfloat16, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq,
+                                         P, stream);
+}
+
+template <typename T>
+static int msda_fused_box_backward(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
+                                   const float* ref, const void* offs, const void* logits, const void* grad_out,
+                                   void* grad_value, void* grad_offs, void* grad_logits, int N, int S, int M, int D,
+                                   int L, int Lq, int P, bool det, void* workspace, void* stream) {
+  return msda_fused_backward<T, 4>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
+                                   static_cast<const T*>(offs), static_cast<const T*>(logits),
+                                   static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
+                                   static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, det, workspace, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_f32(const float* value, const int64_t* spatial_shapes,
+                                                 const int64_t* level_start, const float* ref, const float* offs,
+                                                 const float* logits, const float* grad_out, float* grad_value,
+                                                 float* grad_offs, float* grad_logits, int N, int S, int M, int D,
+                                                 int L, int Lq, int P, void* stream) {
+  return msda_fused_box_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                        grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_f16(const void* value, const int64_t* spatial_shapes,
+                                                 const int64_t* level_start, const float* ref, const void* offs,
+                                                 const void* logits, const void* grad_out, float* grad_value,
+                                                 void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
+                                                 int Lq, int P, void* stream) {
+  return msda_fused_box_backward<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                         grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_bf16(const void* value, const int64_t* spatial_shapes,
+                                                  const int64_t* level_start, const float* ref, const void* offs,
+                                                  const void* logits, const void* grad_out, float* grad_value,
+                                                  void* grad_offs, void* grad_logits, int N, int S, int M, int D,
+                                                  int L, int Lq, int P, void* stream) {
+  return msda_fused_box_backward<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
+                                                grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, false,
+                                                nullptr, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_det_f32(const float* value, const int64_t* spatial_shapes,
+                                                     const int64_t* level_start, const float* ref, const float* offs,
+                                                     const float* logits, const float* grad_out, float* grad_value,
+                                                     float* grad_offs, float* grad_logits, int N, int S, int M, int D,
+                                                     int L, int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_box_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                        grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_det_f16(const void* value, const int64_t* spatial_shapes,
+                                                     const int64_t* level_start, const float* ref, const void* offs,
+                                                     const void* logits, const void* grad_out, void* grad_value,
+                                                     void* grad_offs, void* grad_logits, int N, int S, int M, int D,
+                                                     int L, int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_box_backward<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
+                                         grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
+}
+
+extern "C" int odise_msda_fused_box_backward_det_bf16(const void* value, const int64_t* spatial_shapes,
+                                                      const int64_t* level_start, const float* ref, const void* offs,
+                                                      const void* logits, const void* grad_out, void* grad_value,
+                                                      void* grad_offs, void* grad_logits, int N, int S, int M, int D,
+                                                      int L, int Lq, int P, void* workspace, void* stream) {
+  return msda_fused_box_backward<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
+                                                grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, true,
+                                                workspace, stream);
 }

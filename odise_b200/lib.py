@@ -63,6 +63,15 @@ _SIGS = {
     "odise_msda_fused_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_msda_fused_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_msda_fused_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_box_f32": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_f16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_bf16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_backward_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_backward_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_backward_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
+    "odise_msda_fused_box_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_box_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_msda_fused_box_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -561,9 +570,9 @@ ODISE_ERR_UNSUPPORTED = 10006
 
 
 def _msda_d32_only(fn, S, M, D, L, P):
-    """The shapes the fused backward and the 16-bit fused forward take (d32_ok in msda.cu; their entry points return
-    ODISE_ERR_UNSUPPORTED on any other): D = 32, L*P <= 32 and S*M*D < 2^31.  Raises before any launch, and needs no
-    library, so that the fake implementations of odise_b200.msda's ops refuse the same shapes."""
+    """The shapes the fused backward, the 16-bit fused forward and every box entry point take (d32_ok in msda.cu; their
+    entry points return ODISE_ERR_UNSUPPORTED on any other): D = 32, L*P <= 32 and S*M*D < 2^31.  Raises before any
+    launch, and needs no library, so that the fake implementations of odise_b200.msda's ops refuse the same shapes."""
     if not (D == 32 and L * P <= 32 and S * M * D < 2 ** 31):
         raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
 
@@ -571,9 +580,10 @@ def _msda_d32_only(fn, S, M, D, L, P):
 def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
                        dtype=torch.float32):
     """Checks of the fused entry points: CUDA, contiguous, reference_points float32 and every other tensor of `dtype`,
-    and the layouts of odise_msda_fused_f32 (value [N, S, M, D], reference_points [N, Lq, L, 2], offsets
-    [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P], grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P, spatial_shapes,
-    level_start_index) with the two index tensors as int64 on the value's device."""
+    and the layouts of odise_msda_fused_f32 (value [N, S, M, D], reference_points [N, Lq, L, 2] or boxes [N, Lq, L, 4]
+    with a storage offset that keeps them 16-byte aligned, offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P],
+    grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P,
+    spatial_shapes, level_start_index) with the two index tensors as int64 on the value's device."""
     named = [(value, "value"), (reference_points, "reference_points"), (offsets, "offsets"), (logits, "logits")]
     if grad_output is not None:
         named.append((grad_output, "grad_output"))
@@ -588,25 +598,46 @@ def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_point
                          f"{tuple(offsets.shape)}")
     N, S, M, D = value.shape
     _, Lq, _, L, P, _ = offsets.shape
-    want = {"offsets": (N, Lq, M, L, P, 2), "reference_points": (N, Lq, L, 2), "logits": (N, Lq, M, L * P),
+    rw = 4 if _msda_box(reference_points) else 2
+    want = {"offsets": (N, Lq, M, L, P, 2), "reference_points": (N, Lq, L, rw), "logits": (N, Lq, M, L * P),
             "spatial_shapes": (L, 2), "level_start_index": (L,)}
     if grad_output is not None:
         want["grad_output"] = (N, Lq, M * D)
     for t, nm in named[1:] + [(spatial_shapes, "spatial_shapes"), (level_start_index, "level_start_index")]:
         if tuple(t.shape) != want[nm]:
-            raise OdiseError(f"{nm}: expected shape {want[nm]}, got {tuple(t.shape)}")
+            alt = f" or {want[nm][:3] + (4,)}" if nm == "reference_points" else ""
+            raise OdiseError(f"{nm}: expected shape {want[nm]}{alt}, got {tuple(t.shape)}")
+    if rw == 4 and reference_points.storage_offset() % 4:
+        # a box is one 16-byte load (the entry points return ODISE_ERR_ARG otherwise); checked on the storage offset,
+        # which a fake tensor has too, so that a view into an allocation fails here and not at the launch
+        raise OdiseError("reference_points: box reference points must start 16 bytes into their storage "
+                         f"(storage offset a multiple of 4 floats, got {reference_points.storage_offset()}); pass a "
+                         "copy")
     ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
     ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
     return N, S, M, D, L, Lq, P, ss, ls
 
 
+def _msda_box(reference_points):
+    """True for box reference points [N, Lq, L, 4] (cx, cy, w, h): the odise_msda_fused_box_* entry points."""
+    return reference_points.dim() == 4 and reference_points.shape[-1] == 4
+
+
 def msda_fused_forward(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
     """MSDeformAttn's sampling from the raw linear outputs (odise_msda_fused_f32: softmax over L*P and
-    loc = ref + off / (W_l, H_l) inside the kernel) -> out [N, Lq, M*D] float32.  RuntimeError on CPU, non-contiguous or
-    non-float32 tensors, on shapes that disagree and on a D the kernel does not take."""
+    loc = ref + off / (W_l, H_l) inside the kernel) -> out [N, Lq, M*D] float32.  Box reference points [N, Lq, L, 4]
+    take odise_msda_fused_box_f32 (loc = ref.xy + off / P * ref.wh * 0.5), D = 32, L*P <= 32 and S*M*D < 2^31 only.
+    RuntimeError on CPU, non-contiguous or non-float32 tensors, on shapes that disagree and on a D the kernel does not
+    take."""
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits)
     out = torch.empty(N, Lq, M * D, dtype=torch.float32, device=value.device)
+    if _msda_box(reference_points):
+        fn = "odise_msda_fused_box_f32"
+        _msda_d32_only(fn, S, M, D, L, P)
+        _check(load().odise_msda_fused_box_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
+                                               _ptr(logits), _ptr(out), N, S, M, D, L, Lq, P, _stream()), fn)
+        return out
     _check(load().odise_msda_fused_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
                                        _ptr(logits), _ptr(out), None, None, N, S, M, D, L, Lq, P, _stream()),
            "odise_msda_fused_f32")
@@ -618,10 +649,12 @@ def msda_fused_backward(value, spatial_shapes, level_start_index, reference_poin
     """Backward of msda_fused_forward (odise_msda_fused_backward_f32) -> (grad_value, grad_offsets, grad_logits) shaped
     like value / offsets / logits.  D = 32 and L*P <= 32 only; RuntimeError otherwise and on the input errors of
     msda_fused_forward.  grad_offsets and grad_logits are bit-deterministic; deterministic=True
-    (odise_msda_fused_backward_det_f32) makes grad_value so too."""
+    (odise_msda_fused_backward_det_f32) makes grad_value so too.  Box reference points take
+    odise_msda_fused_box_backward_f32 / _det_f32."""
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output)
-    fn = "odise_msda_fused_backward_det_f32" if deterministic else "odise_msda_fused_backward_f32"
+    box = "box_" if _msda_box(reference_points) else ""
+    fn = f"odise_msda_fused_{box}backward_{'det_' if deterministic else ''}f32"
     _msda_d32_only(fn, S, M, D, L, P)
     grad_value = torch.empty_like(value)
     grad_offs = torch.empty_like(offsets)
@@ -649,12 +682,13 @@ def _msda_16bit_suffix(value):
 def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
     """msda_fused_forward with 16-bit storage (odise_msda_fused_f16 / _bf16, chosen by value.dtype): value, offsets and
     logits float16 or bfloat16 (one dtype), reference_points float32 -> out [N, Lq, M*D] in the value's dtype, one rounding
-    of the fp32 result.  D = 32 and L*P <= 32 only.  RuntimeError on CPU or non-contiguous tensors, on a float32 value,
-    on mixed dtypes, on shapes that disagree and on unsupported shapes."""
+    of the fp32 result.  D = 32 and L*P <= 32 only.  Box reference points [N, Lq, L, 4] take odise_msda_fused_box_f16 /
+    _bf16.  RuntimeError on CPU or non-contiguous tensors, on a float32 value, on mixed dtypes, on shapes that disagree
+    and on unsupported shapes."""
     sfx = _msda_16bit_suffix(value)
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, dtype=value.dtype)
-    fn = "odise_msda_fused_" + sfx
+    fn = "odise_msda_fused_" + ("box_" if _msda_box(reference_points) else "") + sfx
     _msda_d32_only(fn, S, M, D, L, P)
     out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
     rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
@@ -669,11 +703,13 @@ def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, referenc
     grad_logits), each in the value's dtype.  grad_value is accumulated in a float32 buffer and rounded once here;
     grad_offsets and grad_logits are rounded once in the kernel and are bit-deterministic.  grad_output has the value's
     dtype.  Errors as msda_fused_forward_16bit.  deterministic=True (odise_msda_fused_backward_det_f16 / _bf16) sums
-    grad_value in int64 fixed point and the kernels write it in the value's dtype: its bits depend on the inputs only."""
+    grad_value in int64 fixed point and the kernels write it in the value's dtype: its bits depend on the inputs only.
+    Box reference points take odise_msda_fused_box_backward_* (and _det_*)."""
     sfx = _msda_16bit_suffix(value)
     N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                       offsets, logits, grad_output, dtype=value.dtype)
-    fn = ("odise_msda_fused_backward_det_" if deterministic else "odise_msda_fused_backward_") + sfx
+    box = "box_" if _msda_box(reference_points) else ""
+    fn = f"odise_msda_fused_{box}backward_{'det_' if deterministic else ''}{sfx}"
     _msda_d32_only(fn, S, M, D, L, P)
     grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
     grad_offs = torch.empty_like(offsets)

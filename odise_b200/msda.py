@@ -8,7 +8,8 @@ the autograd Function and the nn.Module).
 MSDA exposes the native module's two entry points with its arguments and results, for float32 and float64 CUDA tensors;
 MSDeformAttnFunction is the autograd Function of ops/functions/ms_deform_attn_func.py:32-49 on top of them.
 MSDeformAttnFusedFunction differentiates the fused op (odise_msda_fused_f32 / odise_msda_fused_backward_f32: softmax and
-sampling locations computed inside the kernels; float16 and bfloat16 storage under autocast), and MSDeformAttn is the
+sampling locations computed inside the kernels, for 2-column reference points and for boxes; float16 and bfloat16 storage
+under autocast), and MSDeformAttn is the
 module of ops/modules/ms_deform_attn.py, which takes the fused op where it applies.  All of them run the library's sm_90a
 kernels; there is no CPU path.  Under torch.use_deterministic_algorithms(True) every backward here returns a
 bit-reproducible grad_value (fixed-point sums, lib's deterministic=True); the other gradients are deterministic anyway.
@@ -95,12 +96,13 @@ def _msda_backward_fake(value, spatial_shapes, level_start_index, sampling_loc, 
 
 def _msda_fused_fake_shapes(op, value, spatial_shapes, level_start_index, reference_points, offsets, logits,
                             grad_output=None):
-    """lib's checks of the fused op `op` (forward when grad_output is None) for value's dtype -> (N, Lq, M, D)"""
+    """lib's checks of the fused op `op` (forward when grad_output is None) for value's dtype and reference-point width
+    -> (N, Lq, M, D)"""
     low = value.dtype in _LOW
     N, S, M, D, L, Lq, P, _, _ = lib._msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
                                                         offsets, logits, grad_output,
                                                         dtype=value.dtype if low else torch.float32)
-    if low or grad_output is not None:
+    if low or grad_output is not None or lib._msda_box(reference_points):
         lib._msda_d32_only(op, S, M, D, L, P)
     return N, Lq, M, D
 
@@ -167,15 +169,21 @@ class MSDeformAttnFusedFunction(Function):
     """Autograd through the fused op: forward odise_msda_fused_f32, backward odise_msda_fused_backward_f32, or their
     16-bit forms (odise_msda_fused_f16 / _bf16 and the backward) when value is float16 or bfloat16.
 
-    Inputs: value [N, S, M, D], spatial_shapes [L, 2], level_start_index [L], reference_points [N, Lq, L, 2], offsets
-    [N, Lq, M, L, P, 2] (raw output of the sampling_offsets linear) and logits [N, Lq, M, L*P] (raw output of the
-    attention_weights linear); CUDA tensors, value / offsets / logits float32 or all of one 16-bit dtype,
-    reference_points float32; D = 32 and L*P <= 32 for the backward (and for the 16-bit forward).  Gradients for value,
-    offsets and logits in their dtype; for reference_points only when it requires one, as grad_ref[n, q, l] = sum over
-    (m, p) of grad_offsets * (W_l, H_l), computed in float32."""
+    Inputs: value [N, S, M, D], spatial_shapes [L, 2], level_start_index [L], reference_points [N, Lq, L, 2] or boxes
+    [N, Lq, L, 4] (cx, cy, w, h), offsets [N, Lq, M, L, P, 2] (raw output of the sampling_offsets linear) and logits
+    [N, Lq, M, L*P] (raw output of the attention_weights linear); CUDA tensors, value / offsets / logits float32 or all of
+    one 16-bit dtype, reference_points float32; D = 32 and L*P <= 32 for the backward (and for the 16-bit and the box
+    forward).  Gradients for value, offsets and logits in their dtype.  For 2-column reference_points that require one,
+    grad_ref[n, q, l] = sum over (m, p) of grad_offsets * (W_l, H_l), computed in float32.  Boxes get no gradient here:
+    it cannot be recovered from grad_offsets without dividing by w and h, so forward raises RuntimeError for a box that
+    requires grad (MSDeformAttn sends those to the composed path)."""
 
     @staticmethod
     def forward(ctx, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+        if ctx.needs_input_grad[3] and lib._msda_box(reference_points):
+            raise RuntimeError("MSDeformAttnFusedFunction: box reference points [N, Lq, L, 4] that require grad are not "
+                               "supported by the fused op; detach them or use the composed path "
+                               "(MSDeformAttn with use_fused = False)")
         output = torch.ops.odise_b200.msda_fused_forward(value, spatial_shapes, level_start_index, reference_points,
                                                          offsets, logits)
         ctx.save_for_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits)
@@ -207,10 +215,13 @@ class MSDeformAttn(nn.Module):
     names and shapes (state dicts load both ways), initialisation and forward signature.
 
     forward() runs MSDeformAttnFusedFunction (softmax, sampling locations and bilinear sampling in one kernel, and one
-    kernel for their backward) for float32 CUDA inputs with 2-column reference points, D = d_model / n_heads = 32,
-    n_levels * n_points <= 32 and S * d_model < 2^31.  Every other input (other D, float64, 4-column box reference
-    points, or use_fused = False) takes the reference's composition: softmax and locations in torch ops, then
-    MSDeformAttnFunction.  CPU tensors raise: there is no CPU path.
+    kernel for their backward) for float32 CUDA inputs with 2-column reference points or 4-column boxes,
+    D = d_model / n_heads = 32, n_levels * n_points <= 32 and S * d_model < 2^31.  A box that needs a gradient
+    (grad mode on and reference_points.requires_grad) is the exception: the fused kernels return the gradient of the raw
+    offsets, from which a box's own gradient cannot be recovered without dividing by w and h, so it takes the composed
+    path.  Decoders that detach their boxes between layers (box refinement) stay fused, as does torch.no_grad.  Every
+    other input (other D, float64, or use_fused = False) takes the reference's composition: softmax and locations in
+    torch ops, then MSDeformAttnFunction.  CPU tensors raise: there is no CPU path.
 
     Under torch.autocast, or in a module cast to float16 / bfloat16, value, offsets and logits come out of the Linears in
     16 bits.  Where the fused conditions hold, the 16-bit fused kernels take them as they are (reference points cast to
@@ -278,11 +289,20 @@ class MSDeformAttn(nn.Module):
         low = value.dtype in _LOW
         # float32 needs float32 reference points; a 16-bit value takes them in float32 or 16 bits (cast exactly below)
         ref_ok = reference_points.dtype in ((torch.float32,) + _LOW if low else (torch.float32,))
+        # a box that needs a gradient stays composed (MSDeformAttnFusedFunction has no box gradient)
+        box_grad = reference_points.shape[-1] == 4 and torch.is_grad_enabled() and reference_points.requires_grad
         fused = (self.use_fused and (value.dtype == torch.float32 or low) and offsets.dtype == logits.dtype == value.dtype
-                 and ref_ok and reference_points.shape[-1] == 2 and D == 32 and L * P <= 32 and S * M * D < 2 ** 31)
+                 and ref_ok and not box_grad and D == 32 and L * P <= 32 and S * M * D < 2 ** 31)
         if fused:
-            output = MSDeformAttnFusedFunction.apply(value, input_spatial_shapes, input_level_start_index,
-                                                     reference_points.to(torch.float32).contiguous(), offsets, logits)
+            ref = reference_points.to(torch.float32).contiguous()
+            if ref.shape[-1] == 4:     # here grad mode is off or the box needs no gradient
+                ref = ref.detach()
+                # a view that the box kernels' 16-byte loads cannot read is copied.  Dynamo cannot trace
+                # storage_offset(), so a traced graph leaves the check to the op's fake implementation (lib's validator)
+                if not torch.compiler.is_compiling() and ref.storage_offset() % 4:
+                    ref = ref.clone()
+            output = MSDeformAttnFusedFunction.apply(value, input_spatial_shapes, input_level_start_index, ref, offsets,
+                                                     logits)
         else:
             out_dtype = value.dtype
             if low:                    # sample in float32 (what the reference's grid_sample fallback does under autocast)
