@@ -428,6 +428,45 @@ int odise_mha_d32_ws_f32(const float* q, long long ldq, const float* k, const fl
                          long long ldo, int B, int Tq, int Tk, int heads, float scale, float* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Masked cross-attention for training (Mask2Former CrossAttentionLayer, mask2former_transformer_decoder.py:75-135:
+ * nn.MultiheadAttention with a bool attn_mask), forward and backward of the attention core
+ *   out[q, b, h, :] = softmax_j((s * q[q, b, h, :]) . k[j, b, h, :], blocked -> -inf) v[j, b, h, :],  s = 1/sqrt(D)
+ * on the sequence-first layouts of the in-projections: q and out [Q, B, H*D], k and v [S, B, H*D], contiguous.  D = 32
+ * only (ODISE_ERR_UNSUPPORTED otherwise).  mask: bytes, non-zero = blocked (a torch bool tensor), element (b*H + h, q, j)
+ * at mask[(b*H + h) * mask_bh_stride + q * S + j]: mask_bh_stride = Q*S for [B*H, Q, S], 0 for a [Q, S] mask shared by
+ * every (b, h); NULL = no mask.  _f32 / _f16 / _bf16: q, k, v, out, grad_out and the gradients in float, __half or
+ * __nv_bfloat16 (one type); all arithmetic fp32, every output rounded once.  lse [B*H, Q] float32 = the log-sum-exp of
+ * each row's scores, the only thing the backward needs beyond the inputs and out.  A row whose keys are all blocked
+ * gives what torch's math path gives: a NaN output row (lse = -inf), a NaN grad_q row, and NaN grad_k / grad_v over its
+ * whole (b, h).  The workspace (odise_masked_xattn_workspace_bytes(B, H, Q, S) bytes, 16-byte aligned, any content) holds
+ * fp32 partials: the forward splits the keys into chunks whose number depends on the shape only, and every gradient is
+ * summed in a fixed order without atomics, so out, lse, grad_q, grad_k and grad_v are bit-reproducible.  q / k / v / out /
+ * gradient pointers must be 16-byte (float) or 8-byte (16-bit) aligned (ODISE_ERR_ALIGN).  No host synchronisation and
+ * no allocation (CUDA-graph capturable).  workspace_bytes returns 0 for shapes the entry points refuse. */
+long long odise_masked_xattn_workspace_bytes(int B, int H, int Q, int S);
+int odise_masked_xattn_forward_f32(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                   long long mask_bh_stride, void* out, float* lse, int B, int H, int D, int Q, int S,
+                                   void* workspace, void* stream);
+int odise_masked_xattn_forward_f16(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                   long long mask_bh_stride, void* out, float* lse, int B, int H, int D, int Q, int S,
+                                   void* workspace, void* stream);
+int odise_masked_xattn_forward_bf16(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                    long long mask_bh_stride, void* out, float* lse, int B, int H, int D, int Q, int S,
+                                    void* workspace, void* stream);
+int odise_masked_xattn_backward_f32(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                    long long mask_bh_stride, const void* out, const float* lse, const void* grad_out,
+                                    void* grad_q, void* grad_k, void* grad_v, int B, int H, int D, int Q, int S,
+                                    void* workspace, void* stream);
+int odise_masked_xattn_backward_f16(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                    long long mask_bh_stride, const void* out, const float* lse, const void* grad_out,
+                                    void* grad_q, void* grad_k, void* grad_v, int B, int H, int D, int Q, int S,
+                                    void* workspace, void* stream);
+int odise_masked_xattn_backward_bf16(const void* q, const void* k, const void* v, const uint8_t* mask,
+                                     long long mask_bh_stride, const void* out, const float* lse, const void* grad_out,
+                                     void* grad_q, void* grad_k, void* grad_v, int B, int H, int D, int Q, int S,
+                                     void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

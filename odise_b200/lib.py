@@ -72,6 +72,13 @@ _SIGS = {
     "odise_msda_fused_box_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_msda_fused_box_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
     "odise_msda_fused_box_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
+    "odise_masked_xattn_workspace_bytes": [c_int] * 4,       # returns long long (set in load())
+    "odise_masked_xattn_forward_f32": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_masked_xattn_forward_f16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_masked_xattn_forward_bf16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_masked_xattn_backward_f32": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_masked_xattn_backward_f16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_masked_xattn_backward_bf16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -181,6 +188,7 @@ def load():
         fn.argtypes = args
         fn.restype = c_int
     lib.odise_msda_det_workspace_bytes.restype = c_longlong
+    lib.odise_masked_xattn_workspace_bytes.restype = c_longlong
     _lib = lib
     return lib
 
@@ -723,6 +731,86 @@ def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, referenc
     rc = getattr(load(), fn)(*args, _stream())
     _check(rc, fn)
     return grad_value.to(value.dtype), grad_offs, grad_logits
+
+
+_XATTN_SFX = {torch.float32: "f32", torch.float16: "f16", torch.bfloat16: "bf16"}
+
+
+def _xattn_shapes(q, k, v, mask, heads, out=None, lse=None, grad_out=None):
+    """Checks of the masked cross-attention entry points, without data and without the library (the fake
+    implementations of odise_b200.masked_attn's ops call it too): q [Q, B, E], k and v [S, B, E], E = heads * 32, CUDA,
+    contiguous, one dtype of float32 / float16 / bfloat16; mask None or a contiguous CUDA bool [B*heads, Q, S] or
+    [Q, S]; for the backward out and grad_out like q and lse [B*heads, Q] float32.  -> (Q, B, E, S, mask_bh_stride)"""
+    named = [(q, "q"), (k, "k"), (v, "v")] + [(t, n) for t, n in ((out, "out"), (grad_out, "grad_out")) if t is not None]
+    if q.dtype not in _XATTN_SFX:
+        raise OdiseError(f"q: expected float32, float16 or bfloat16, got {q.dtype}")
+    for t, nm in named:
+        if not t.is_cuda:
+            raise OdiseError(f"{nm} must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise OdiseError(f"{nm} tensor has to be contiguous")
+        _req(t, q.dtype, nm)
+        if t.dim() != 3:
+            raise OdiseError(f"{nm}: expected a 3-D tensor, got {tuple(t.shape)}")
+    Q, B, E = q.shape
+    S = k.shape[0]
+    if heads <= 0 or E % heads:
+        raise OdiseError(f"embed dim {E} is not divisible by heads = {heads}")
+    if E // heads != 32:
+        raise OdiseError(f"masked cross-attention: head dim {E // heads} not supported (32 only)")
+    for t, nm, want in ((k, "k", (S, B, E)), (v, "v", (S, B, E)), (out, "out", (Q, B, E)),
+                        (grad_out, "grad_out", (Q, B, E))):
+        if t is not None and tuple(t.shape) != want:
+            raise OdiseError(f"{nm}: expected shape {want}, got {tuple(t.shape)}")
+    if S <= 0 or Q <= 0 or B <= 0:
+        raise OdiseError(f"empty sequence: Q = {Q}, S = {S}, B = {B}")
+    if B * heads > 65535 or (S + 63) // 64 > 65535:
+        raise OdiseError(f"masked cross-attention: B*heads = {B * heads} or S = {S} too large")
+    if lse is not None:
+        if not lse.is_cuda or lse.dtype != torch.float32 or tuple(lse.shape) != (B * heads, Q) or not lse.is_contiguous():
+            raise OdiseError(f"lse: expected a contiguous CUDA float32 tensor of shape {(B * heads, Q)}")
+    stride = 0
+    if mask is not None:
+        if not mask.is_cuda or mask.dtype != torch.bool or not mask.is_contiguous():
+            raise OdiseError("mask: expected a contiguous CUDA bool tensor (True = blocked)")
+        if tuple(mask.shape) == (B * heads, Q, S):
+            stride = Q * S
+        elif tuple(mask.shape) != (Q, S):
+            raise OdiseError(f"mask: expected shape {(B * heads, Q, S)} or {(Q, S)}, got {tuple(mask.shape)}")
+    return Q, B, E, S, stride
+
+
+def _xattn_workspace(B, H, Q, S, device):
+    """workspace of the masked cross-attention entry points (odise_masked_xattn_workspace_bytes), from torch's allocator"""
+    return torch.empty(int(load().odise_masked_xattn_workspace_bytes(B, H, Q, S)), dtype=torch.uint8, device=device)
+
+
+def masked_xattn_forward(q, k, v, mask, heads):
+    """Masked cross-attention core of nn.MultiheadAttention (odise_masked_xattn_forward_f32 / _f16 / _bf16 by q.dtype):
+    q [Q, B, heads*32], k and v [S, B, heads*32] (the in-projection outputs, sequence first), mask None or bool
+    [B*heads, Q, S] / [Q, S] with True = blocked -> (out [Q, B, heads*32] in q's dtype, lse [B*heads, Q] float32).
+    RuntimeError on CPU, non-contiguous or mixed-dtype tensors, shapes that disagree and a head dim other than 32."""
+    Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads)
+    out = torch.empty_like(q)
+    lse = torch.empty(B * heads, Q, dtype=torch.float32, device=q.device)
+    ws = _xattn_workspace(B, heads, Q, S, q.device)
+    fn = "odise_masked_xattn_forward_" + _XATTN_SFX[q.dtype]
+    _check(getattr(load(), fn)(_ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out), _ptr(lse), B, heads, 32, Q, S,
+                               _ptr(ws), _stream()), fn)
+    return out, lse
+
+
+def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
+    """Backward of masked_xattn_forward (odise_masked_xattn_backward_*) -> (grad_q, grad_k, grad_v) shaped and typed like
+    q / k / v.  grad_out has q's dtype.  Every result is bit-reproducible (fixed-order sums, no atomics).  Errors as
+    masked_xattn_forward, and for out / lse / grad_out of the wrong shape or dtype."""
+    Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads, out=out, lse=lse, grad_out=grad_out)
+    gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    ws = _xattn_workspace(B, heads, Q, S, q.device)
+    fn = "odise_masked_xattn_backward_" + _XATTN_SFX[q.dtype]
+    _check(getattr(load(), fn)(_ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out), _ptr(lse), _ptr(grad_out),
+                               _ptr(gq), _ptr(gk), _ptr(gv), B, heads, 32, Q, S, _ptr(ws), _stream()), fn)
+    return gq, gk, gv
 
 
 class nvtx:
