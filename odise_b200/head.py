@@ -328,15 +328,24 @@ class HeadEngine:
             raise lib.OdiseError(f"the decoder has {nl} feature levels, got {len(shapes)} maps")
         for lvl, (h, w) in enumerate(shapes):
             hw = h * w
+            hw8 = (hw + 7) // 8 * 8                # keys per image in the K / V^T planes: the attention's TMA row stride
             nk = self.W[f"dec.k{lvl}"].rows // CP                         # layers reading this level (i % nl == lvl)
-            k = Planes.empty(B * hw, nk * CP, dev, lo=self.lo)           # [B*hw, nk layers x 8 heads x 64]
+            k = Planes.empty(B * hw8, nk * CP, dev, lo=self.lo)          # [B*hw8, nk layers x 8 heads x 64]
             lib.gemm(kin_p.row_slice(starts[lvl], hw), self.W[f"dec.k{lvl}"], M=hw, N=nk * CP, K=256, nmma=self.nmma,
-                     batch=B, a_bs=S * kin_p.ld, bias=self.F[f"dec.k{lvl}.b"], out_planes=k, outp_bs=hw * k.ld)
-            # V^T [nk*CP, B*hw]: swapped operands, image z lands at column offset z*hw
-            vt = Planes.empty(nk * CP, B * hw, dev, lo=self.lo, f16=self.lo)
+                     batch=B, a_bs=S * kin_p.ld, bias=self.F[f"dec.k{lvl}.b"], out_planes=k, outp_bs=hw8 * k.ld)
+            # V^T [nk*CP, B*hw8]: swapped operands, image z lands at column offset z*hw8
+            vt = Planes.empty(nk * CP, B * hw8, dev, lo=self.lo, f16=self.lo)
             lib.gemm(self.W[f"dec.v{lvl}"], vin_p.row_slice(starts[lvl], hw), M=nk * CP, N=hw, K=256, nmma=self.nmma,
-                     batch=B, b_bs=S * vin_p.ld, bias_m=self.F[f"dec.v{lvl}.b"], out_planes=vt, outp_bs=hw)
-            K.append(k)
+                     batch=B, b_bs=S * vin_p.ld, bias_m=self.F[f"dec.v{lvl}.b"], out_planes=vt, outp_bs=hw8)
+            if hw8 != hw:   # s5 of a 64a x 64b input with a*b odd: the GEMMs never write the pad keys, which the kernel
+                # gives P = 0, and 0 * NaN from uninitialised memory would still be NaN in the P V product
+                for plane in (k.hi, k.lo):
+                    if plane is not None:
+                        plane.view(B, hw8, k.ld)[:, hw:].zero_()
+                for plane in (vt.hi, vt.lo):
+                    if plane is not None:
+                        plane.view(nk * CP, B, hw8)[:, :, hw:].zero_()
+            K.append((k, hw8))
             V.append(vt)
         fm = (lambda i: None) if forced_masks is None else (lambda i: forced_masks[i])
         output = g["query0"]
@@ -348,13 +357,15 @@ class HeadEngine:
         for i in range(self.n_dec):
             lvl, slot = i % nl, i // nl
             hw = shapes[lvl][0] * shapes[lvl][1]
+            k, hw8 = K[lvl]
             n = f"dec.l{i}."
-            # masked cross-attention (mask2former_transformer_decoder.py:98-110, odise.py:683-692)
+            # masked cross-attention (mask2former_transformer_decoder.py:98-110, odise.py:683-692); the mask bits stay
+            # [B, Q, ceil(hw / 32)] words, only the key planes are strided by hw8
             _, qin_p = ops.add_split(output, qe, b_rows=Q, lo=self.lo)
             qc = Planes.empty(B * Q, CP, dev, lo=self.lo)
             self._gemm(qin_p, n + "cq", out_planes=qc)
-            _, o_p = ops.attention_tc(qc, K[lvl].col_slice(slot * CP, CP), V[lvl].row_slice(slot * CP, CP), B, M_HEADS,
-                                      D_HEAD, Q, hw, scale, self.nmma, tk_stride=hw, mask_bits=bits, row_any=row_any)
+            _, o_p = ops.attention_tc(qc, k.col_slice(slot * CP, CP), V[lvl].row_slice(slot * CP, CP), B, M_HEADS,
+                                      D_HEAD, Q, hw, scale, self.nmma, tk_stride=hw8, mask_bits=bits, row_any=row_any)
             t = ops.empty(B * Q, 256, dev)
             self._gemm(o_p, n + "co", residual=output, out=t)
             output, _ = self._ln(t, n + "cn", want_f32=True, want_planes=False)

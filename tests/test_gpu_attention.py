@@ -62,15 +62,23 @@ def test_softmax_split(cuda):
 
 
 @pytest.mark.parametrize("nmma", [3, 1])
-@pytest.mark.parametrize("cfg", [(2, 100, 32 * 32, 64, 64), (1, 100, 64 * 64, 256, 256), (2, 37, 8 * 8, 32, 32)])
+@pytest.mark.parametrize("cfg", [(2, 100, 64, 64, 32, 32, None), (1, 100, 256, 256, 64, 64, None), (2, 37, 32, 32, 8, 8, None),
+                                 # the decoder at a portrait 576 x 448 input: masks at H/4 x W/4 = 144 x 112 resized to its
+                                 # H/32, H/16 and H/8 levels; the s5 level's 252 keys per image sit at a stride of 256
+                                 (2, 100, 144, 112, 18, 14, 256), (2, 100, 144, 112, 36, 28, None),
+                                 (1, 100, 144, 112, 72, 56, None),
+                                 # landscape, 252 keys per image at a stride of 392 (140 pad rows per image)
+                                 (2, 37, 112, 144, 14, 18, 392)])
 def test_masked_attention_tc_d32(cuda, nmma, cfg):
     """Mask2Former masked cross-attention (odise.py:683-692, 760-774) on the wgmma kernel: head dim 32, mask bits from
-    odise_attn_mask_bits_f32, fully-masked rows attend everywhere."""
+    odise_attn_mask_bits_f32 (masks Hm x Wm resized to the key level Hl x Wl), fully-masked rows attend everywhere.
+    TkS = rows per image in the key / value planes (None: Tk); its pad rows hold large finite junk that must be masked."""
     import torch.nn.functional as F
     from odise_b200 import lib, ops
-    B, Tq, Tk, Hm, Wm = cfg
+    B, Tq, Hm, Wm, Hl, Wl, TkS = cfg
+    Tk = Hl * Wl
+    TkS = TkS or Tk
     heads, d, HS = 8, 32, 64
-    Hl = Wl = int(Tk ** 0.5)
     g = torch.Generator().manual_seed(Tk + Tq)
     q = torch.randn(B, Tq, heads, d, generator=g).to(cuda)
     k = torch.randn(B, Tk, heads, d, generator=g).to(cuda)
@@ -81,18 +89,20 @@ def test_masked_attention_tc_d32(cuda, nmma, cfg):
     bits, row_any = ops.attn_mask_bits(ml, B, Tq, Hm, Wm, Hl, Wl)
     qp = torch.zeros(B * Tq, heads, HS, device=cuda)
     qp[:, :, :d] = q.view(B * Tq, heads, d)
-    kp = torch.zeros(B * Tk, heads, HS, device=cuda)
-    kp[:, :, :d] = k.view(B * Tk, heads, d)
-    vt = torch.zeros(heads, HS, B * Tk, device=cuda)
-    vt[:, :d] = v.view(B * Tk, heads, d).permute(1, 2, 0)
+    kp = torch.zeros(B, TkS, heads, HS, device=cuda)
+    kp[:, :Tk, :, :d] = k
+    kp[:, Tk:] = 7.0                     # pad keys must be masked, not merely zero
+    vt = torch.zeros(heads, HS, B, TkS, device=cuda)
+    vt[:, :d, :, :Tk] = v.permute(2, 3, 0, 1)
+    vt[:, :, :, Tk:] = 1e3               # finite: exp(-inf) = 0 must zero them, 0 * 1e3 stays 0
     scale = d ** -0.5
-    out, _ = ops.attention_tc(lib.split(qp.view(B * Tq, -1)), lib.split(kp.view(B * Tk, -1)), lib.split(vt.view(heads * HS, -1), f16=nmma == 3),
-                              B, heads, d, Tq, Tk, scale, nmma, want_f32=True, want_planes=False, tk_stride=Tk,
-                              mask_bits=bits, row_any=row_any)
+    out, _ = ops.attention_tc(lib.split(qp.view(B * Tq, -1)), lib.split(kp.view(B * TkS, -1)),
+                              lib.split(vt.view(heads * HS, B * TkS), f16=nmma == 3), B, heads, d, Tq, Tk, scale, nmma,
+                              want_f32=True, want_planes=False, tk_stride=TkS, mask_bits=bits, row_any=row_any)
     torch.cuda.synchronize()
     am = F.interpolate(ml, size=(Hl, Wl), mode="bilinear", align_corners=False).sigmoid().flatten(2) < 0.5
     am[torch.where(am.sum(-1) == am.shape[-1])] = False
     s = torch.einsum("bqhd,bkhd->bhqk", q.double(), k.double()) * scale
     s = s.masked_fill(am[:, None], float("-inf"))
     ref = torch.einsum("bhqk,bkhd->bqhd", s.softmax(-1), v.double()).reshape(B * Tq, heads * d)
-    assert _rel(out, ref) < (TOL3 if nmma == 3 else 3e-2)
+    assert _rel(out, ref) < (TOL3 if nmma == 3 else 3e-2)          # fp64 masked attention: P rounding model (top of file)

@@ -80,17 +80,36 @@ def test_geglu_add_upsample_copy(cuda):
 
 
 @pytest.mark.parametrize("cfg", [(2, 8, 8, 16, 16, 64, 1), (1, 16, 16, 64, 64, 32, 1), (2, 64, 64, 16, 16, 8, 0),
-                                 (1, 16, 16, 64, 64, 8, 0), (1, 32, 32, 32, 32, 16, 0), (1, 256, 256, 128, 128, 4, 1)])
+                                 (1, 16, 16, 64, 64, 8, 0), (1, 32, 32, 32, 32, 16, 0), (1, 256, 256, 128, 128, 4, 1),
+                                 # the pixel decoder's FPN add (head.py::pixel_decoder): s3 rows of the [B, S, 256] encoder
+                                 # memory (after the s5 and s4 rows) bilinearly added into s2, portrait 576 x 448 input
+                                 (2, 72, 56, 144, 112, 256, 1, 18 * 14 + 36 * 28),
+                                 (2, 12, 20, 24, 40, 64, 1, 37), (1, 9, 7, 18, 14, 32, 1, 5), (2, 7, 9, 16, 20, 8, 1, 3)])
 def test_resize(cuda, cfg):
-    B, Hs, Ws, Hd, Wd, C, bil = cfg
+    """cfgs with an 8th field (rows before the level in each image's source block) run ops.resize_nhwc with a per-image
+    source stride and accumulate=True into a non-zero destination; reference F.interpolate + add in fp64, 1e-6."""
+    B, Hs, Ws, Hd, Wd, C, bil = cfg[:7]
     g = torch.Generator().manual_seed(Hs + Hd)
     x = torch.randn(B, Hs, Ws, C, generator=g).to(cuda)
-    y = torch.zeros(B, Hd, Wd, C, device=cuda)
-    _call("odise_resize_nhwc_f32", x.data_ptr(), C, y.data_ptr(), C, B, Hs, Ws, Hd, Wd, C, bil, 0)
     xn = x.permute(0, 3, 1, 2)
-    ref = F.interpolate(xn, size=(Hd, Wd), mode="bilinear", align_corners=False) if bil else \
+    ref = F.interpolate(xn.double(), size=(Hd, Wd), mode="bilinear", align_corners=False) if bil else \
         F.interpolate(xn, size=(Hd, Wd))
-    assert _rel(y, ref.permute(0, 2, 3, 1)) < 1e-6
+    ref = ref.permute(0, 2, 3, 1)
+    if len(cfg) == 7:
+        y = torch.zeros(B, Hd, Wd, C, device=cuda)
+        _call("odise_resize_nhwc_f32", x.data_ptr(), C, y.data_ptr(), C, B, Hs, Ws, Hd, Wd, C, bil, 0)
+    else:
+        from odise_b200 import ops
+        r0 = cfg[7]
+        S = r0 + Hs * Ws + 11                          # rows per image of the source block: other levels around this one
+        src = torch.full((B, S, C), 1e4, device=cuda)  # finite junk outside the level: read only through a wrong stride
+        src[:, r0:r0 + Hs * Ws] = x.reshape(B, Hs * Ws, C)
+        y0 = torch.randn(B, Hd, Wd, C, generator=g).to(cuda)
+        y = y0.clone()
+        ops.resize_nhwc(src.view(B * S, C)[r0:], B, Hs, Ws, Hd, Wd, True, dst=y.view(B * Hd * Wd, C), accumulate=True,
+                        src_bs=S * C)
+        ref = ref + y0.double()
+    assert _rel(y, ref) < 1e-6
 
 
 @pytest.mark.parametrize("cfg", [(2, 9, 9, 4, 1, 1, 1), (1, 16, 16, 320, 2, 1, 1), (1, 16, 16, 128, 2, 0, 1), (2, 8, 8, 3, 1, 1, 1)])
@@ -157,11 +176,36 @@ def test_mask_pool_helpers(cuda):
     assert torch.allclose(pooled, sums / (cnt[..., None] + 1e-8), rtol=1e-6)
 
 
-@pytest.mark.parametrize("cfg", [(2, 100, 32 * 32, 256, 256), (1, 100, 128 * 128, 256, 256), (2, 100, 100, 0, 0), (1, 37, 65, 0, 0)])
+def check_mask_bits(bits, rowany, ml, Hl, Wl):
+    """odise_attn_mask_bits_f32 output vs the reference recipe (F.interpolate bilinear, sigmoid < 0.5 = blocked), bit for
+    bit.  A bit may differ only where the interpolated logit lies within 1e-6 of 0 (where the sigmoid < 0.5 decision of
+    two fp32 evaluations can tie differently), and fewer than 1e-4 of the bits may fall in that band.  Pad bits of the last
+    word must be 0; row_any = some key is allowed."""
+    B, Tq = ml.shape[:2]
+    Tk = Hl * Wl
+    li = F.interpolate(ml, size=(Hl, Wl), mode="bilinear", align_corners=False).flatten(2)
+    want = ~(li.sigmoid() < 0.5)
+    words = bits.view(B, Tq, -1)
+    assert words.shape[-1] == (Tk + 31) // 32
+    got = ((words[..., None] >> torch.arange(32, device=bits.device, dtype=torch.int32)) & 1).flatten(2).bool()
+    assert not got[..., Tk:].any()                                          # ragged last word: pad bits clear
+    got = got[..., :Tk]
+    band = li.abs() <= 1e-6
+    assert band.float().mean().item() < 1e-4, band.float().mean().item()
+    assert torch.equal(got | band, want | band)                             # bit for bit outside the tie band
+    assert torch.equal(rowany.view(B, Tq) != 0, got.any(-1))
+
+
+@pytest.mark.parametrize("cfg", [(2, 100, 32 * 32, 256, 256), (1, 100, 128 * 128, 256, 256), (2, 100, 100, 0, 0), (1, 37, 65, 0, 0),
+                                 # the decoder's masks at H/4 x W/4 resized to its H/32 and H/16 levels, portrait 576 x 448
+                                 # (252 and 1008 keys: ragged last bit words), landscape 256 x 384, and an odd 7 x 9 level
+                                 (2, 100, 18 * 14, 144, 112, 18, 14), (2, 100, 36 * 28, 144, 112, 36, 28),
+                                 (2, 100, 8 * 12, 64, 96, 8, 12), (1, 37, 7 * 9, 28, 36, 7, 9)])
 def test_mha_d32(cuda, cfg):
     """odise_attn_mask_bits_f32 + odise_mha_d32_f32 vs the reference recipe: bilinear resize, sigmoid<0.5 bool mask,
-    fully-masked rows unmasked (odise.py:683,760-774), then softmax attention with -inf bias."""
-    B, Tq, Tk, Hm, Wm = cfg
+    fully-masked rows unmasked (odise.py:683,760-774), then softmax attention with -inf bias.  (Hl, Wl) is the level the
+    mask is resized to (square sqrt(Tk) when not given)."""
+    B, Tq, Tk, Hm, Wm = cfg[:5]
     heads, d = 8, 32
     g = torch.Generator().manual_seed(Tk)
     q = torch.randn(B, Tq, heads * d, generator=g).to(cuda)
@@ -172,12 +216,14 @@ def test_mha_d32(cuda, cfg):
     bias = None
     bits = rowany = None
     if Hm:
-        Hl = Wl = int(Tk ** 0.5)
+        Hl, Wl = cfg[5:] if len(cfg) > 5 else (int(Tk ** 0.5),) * 2
+        assert Hl * Wl == Tk
         ml = (torch.randn(B, Tq, Hm, Wm, generator=g) * 3 - 2.5).to(cuda)
         ml[0, 3] = -5.0          # a fully masked row -> must attend everywhere
         bits = torch.empty(B, Tq, (Tk + 31) // 32, dtype=torch.int32, device=cuda)
         rowany = torch.empty(B, Tq, dtype=torch.int32, device=cuda)
         _call("odise_attn_mask_bits_f32", ml.data_ptr(), bits.data_ptr(), rowany.data_ptr(), B, Tq, Hm, Wm, Hl, Wl)
+        check_mask_bits(bits, rowany, ml, Hl, Wl)
         am = F.interpolate(ml, size=(Hl, Wl), mode="bilinear", align_corners=False).sigmoid().flatten(2) < 0.5
         am[torch.where(am.sum(-1) == am.shape[-1])] = False
         assert rowany[0, 3].item() == 0

@@ -144,28 +144,41 @@ def test_vocabulary_from_tokens(cuda, world):
 @torch.no_grad()
 def test_category_odise_plugin_ragged_batch(cuda, world):
     """B200CategoryODISE: two images of different, non-64-divisible sizes in one batch, outputs at the datasets' original
-    sizes; checked against the oracle post-processing applied to the engine's own logits."""
+    sizes; checked against the oracle post-processing applied to the engine's own logits.  The batch pads to 512 x 640."""
+    _plugin_ragged_batch(cuda, world, ((500, 620), (470, 640)), ((250, 310), (600, 817)), (512, 640))
+
+
+@torch.no_grad()
+def test_category_odise_plugin_ragged_batch_portrait(cuda, world):
+    """the same with a portrait batch that pads to 576 x 448: s5 18 x 14 = 252 keys per image in the decoder's first
+    cross-attention"""
+    _plugin_ragged_batch(cuda, world, ((560, 430), (576, 400)), ((280, 215), (720, 500)), (576, 448))
+
+
+def _plugin_ragged_batch(cuda, world, sizes, outs, padded):
     from odise_b200.plugin import B200CategoryODISE
     from oracle import postprocess as opp
     eng = world["eng"]
     g = torch.Generator().manual_seed(21)
-    ims = [torch.randint(0, 256, (3, 500, 620), generator=g, dtype=torch.uint8),
-           torch.randint(0, 256, (3, 470, 640), generator=g, dtype=torch.uint8)]
-    req = [dict(image=ims[0], height=250, width=310), dict(image=ims[1], height=600, width=817)]
+    ims = [torch.randint(0, 256, (3, h, w), generator=g, dtype=torch.uint8) for h, w in sizes]
+    req = [dict(image=im, height=h, width=w) for im, (h, w) in zip(ims, outs)]
     model = B200CategoryODISE(eng).eval()
     res = model(req)
     torch.cuda.synchronize()
     assert len(res) == 2
-    assert res[0]["sem_seg"].shape == (20, 250, 310) and res[1]["sem_seg"].shape == (20, 600, 817)
-    assert res[0]["panoptic_seg"][0].shape == (250, 310) and res[1]["panoptic_seg"][0].shape == (600, 817)
-    # re-run the network part to get the raw outputs the plugin post-processed (padded batch 512 x 640)
-    net = torch.zeros(2, 3, 512, 640, dtype=torch.uint8)
-    net[0, :, :500, :620], net[1, :, :470, :640] = ims[0], ims[1]
-    out = eng.step(2, 512, 640, images_u8=net.to(cuda), clip_images=net[:, :, :500, :640].contiguous().to(cuda))
+    for r, hw in zip(res, outs):
+        assert r["sem_seg"].shape == (20, *hw) and r["panoptic_seg"][0].shape == hw
+    # re-run the network part to get the raw outputs the plugin post-processed (the padded batch)
+    ph, pw = padded
+    mh, mw = max(h for h, _ in sizes), max(w for _, w in sizes)
+    net = torch.zeros(2, 3, ph, pw, dtype=torch.uint8)
+    for i, (h, w) in enumerate(sizes):
+        net[i, :, :h, :w] = ims[i]
+    out = eng.step(2, ph, pw, images_u8=net.to(cuda), clip_images=net[:, :, :mh, :mw].contiguous().to(cuda))
     things = list(range(0, 20, 2))
     for i, (r, rq) in enumerate(zip(res, req)):
         cls, masks = out["pred_logits"][i].cpu(), out["pred_masks"][i:i + 1].cpu()
-        up = opp.sem_seg_postprocess(opp.upsample_masks(masks, (512, 640))[0], ims[i].shape[-2:], rq["height"], rq["width"])
+        up = opp.sem_seg_postprocess(opp.upsample_masks(masks, padded)[0], ims[i].shape[-2:], rq["height"], rq["width"])
         sem = opp.semantic_inference(cls, up)
         assert ((r["sem_seg"].cpu().double() - sem.double()).abs().max() / sem.abs().max()).item() < 1e-3
         pan, info = opp.panoptic_inference(cls, up, 20, things)
@@ -191,8 +204,24 @@ def test_c1_end_to_end_mask_logits_and_class_scores(cuda, world, record):
     odise.py:951; MaskCLIP patch mask >= 0.5, clip.py:291-321) are teacher-forced with the ORACLE's mask logits — everything
     continuous is computed independently by both sides from the uint8 image — and the un-forced decisions are compared
     separately as a bit-flip rate."""
+    _end_to_end(cuda, world, record, world["img"], "512^2")
+
+
+@torch.no_grad()
+def test_c1_end_to_end_portrait_576x448(cuda, world, record):
+    """The C1 comparison (same oracle, same three 1e-3 bars, same flip bound) on a 576 x 448 portrait image: two vertically
+    stacked, overlapping 448^2 crops; s5 18 x 14 = 252 keys, not a multiple of 8, in the decoder's first cross-attention;
+    MaskCLIP masks of 144 x 112."""
+    from odise_b200.backbone import BackboneEngine
+    assert BackboneEngine.crop_grid(576, 448) == ([(0, 0), (128, 0)], 448)
+    img = torch.randint(0, 256, (1, 3, 576, 448), generator=torch.Generator().manual_seed(82), dtype=torch.uint8)
+    _end_to_end(cuda, world, record, img, "576 x 448")
+
+
+def _end_to_end(cuda, world, record, img, label):
     from oracle import clip as oclip, compose, m2f
-    sd, eng, img = world["sd"], world["eng"], world["img"]
+    sd, eng = world["sd"], world["eng"]
+    H, W = img.shape[-2:]
     mods = compose.load_modules(sd)
     img01 = img.float() / 255.0
     feats = compose.slide_forward(sd, mods, img01, UNCOND17())
@@ -206,22 +235,24 @@ def test_c1_end_to_end_mask_logits_and_class_scores(cuda, world, record):
     # engine, thresholds forced to the oracle's decisions
     dimg = img.to(cuda)
     eng.use_vocabulary("v20")
-    f_e = eng.backbone.forward(1, 512, 512, images_u8=dimg)
+    f_e = eng.backbone.forward(1, H, W, images_u8=dimg)
     pd = eng.head.pixel_decoder(f_e, 1)
     forced = [m.reshape(1, 100, -1).contiguous().to(cuda) for m in ref_masks]
     heads = eng.head.transformer_decoder(pd, 1, forced_masks=forced)
     cat = eng.head.score(heads[-1]["mask_embed"], "v20").view(1, 100, -1)
-    got = eng.clip_head.forward("v20", dimg, 1, 512, 512, ref["pred_masks"].to(cuda).contiguous(), cat)
+    got = eng.clip_head.forward("v20", dimg, 1, H, W, ref["pred_masks"].to(cuda).contiguous(), cat)
     torch.cuda.synchronize()
+    assert ref["pred_masks"].shape[-2:] == (H // 4, W // 4)
     e_mask = _rel(heads[-1]["pred_masks"].view_as(ref["pred_masks"]).cpu(), ref["pred_masks"])
     e_cat = _rel(cat.cpu(), cat_ref)
     e_cls = _rel(got["pred_logits"].cpu(), want_cls)
     # un-forced run: how many discrete decisions differ (reported, bounded loosely: they are discontinuities, not errors)
-    out = eng.step(1, 512, 512, images_u8=dimg)
+    out = eng.step(1, H, W, images_u8=dimg)
     flips = [((h["pred_masks"].view_as(r).cpu() > 0) != (r > 0)).float().mean().item()
              for h, r in zip(out["aux"] + [dict(pred_masks=out["pred_masks"])], ref_masks)]
-    record(f"C1 end to end (512^2, Q=100, 20 classes): final mask logits rel {e_mask:.2e}, category scores rel {e_cat:.2e}, "
+    record(f"C1 end to end ({label}, Q=100, 20 classes): final mask logits rel {e_mask:.2e}, category scores rel {e_cat:.2e}, "
            f"merged class scores rel {e_cls:.2e}; un-forced sign flips per head {['%.1e' % f for f in flips]}")
+    # oracle (compose + m2f + MaskCLIP), 1e-3 relative on each of the three outputs
     assert e_mask < 1e-3 and e_cat < 1e-3 and e_cls < 1e-3, (e_mask, e_cat, e_cls)
     assert max(flips) < 1e-2
 

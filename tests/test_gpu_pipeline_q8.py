@@ -39,6 +39,12 @@ def test_q8_c1_end_to_end(cuda, world_q8, record):
     P.test_c1_end_to_end_mask_logits_and_class_scores(cuda, world_q8, rec)
 
 
+def test_q8_c1_end_to_end_portrait_576x448(cuda, world_q8, record):
+    def rec(line):
+        record("[F16Q8] " + line)
+    P.test_c1_end_to_end_portrait_576x448(cuda, world_q8, rec)
+
+
 def test_q8_full_size_batch4_1024_paste(cuda, world_q8, record):
     def rec(line):
         record("[F16Q8] " + line)

@@ -21,7 +21,8 @@ def _case(seed, B, Q, K, h, w):
     return cls, masks
 
 
-@pytest.mark.parametrize("cfg", [(1, 2, 20, 7, 24, 32, 4), (2, 1, 100, 150, 64, 64, 4), (3, 2, 50, 19, 32, 48, 2)])
+@pytest.mark.parametrize("cfg", [(1, 2, 20, 7, 24, 32, 4), (2, 1, 100, 150, 64, 64, 4), (3, 2, 50, 19, 32, 48, 2),
+                                 (7, 2, 20, 7, 32, 24, 4), (8, 1, 50, 19, 36, 28, 4)])          # portrait: h > w
 def test_postprocess(cuda, cfg):
     from odise_b200.postprocess import PostProcessor
     from oracle import postprocess as opp
@@ -48,7 +49,8 @@ def test_postprocess(cuda, cfg):
     assert n_nonempty > 0
 
 
-@pytest.mark.parametrize("cfg", [(4, 2, 20, 7, 24, 32, 4, 50), (5, 1, 100, 150, 64, 64, 4, 100), (6, 1, 5, 3, 16, 16, 2, 100)])
+@pytest.mark.parametrize("cfg", [(4, 2, 20, 7, 24, 32, 4, 50), (5, 1, 100, 150, 64, 64, 4, 100), (6, 1, 5, 3, 16, 16, 2, 100),
+                                 (10, 2, 20, 7, 32, 24, 4, 50), (11, 1, 5, 3, 20, 12, 2, 100)])  # portrait: h > w
 def test_instance_inference(cuda, cfg):
     """MaskFormer.instance_inference (maskformer_model.py:344-380): top-k (query, class) pairs, mask-weighted scores."""
     from odise_b200.postprocess import PostProcessor
@@ -82,10 +84,18 @@ def test_instance_inference(cuda, cfg):
 def test_postprocess_with_padding_and_resize(cuda):
     """odise.py:326-347: masks upsampled to the padded input, cropped to the image, resized to the dataset's original
     size (sem_seg_postprocess) BEFORE semantic / panoptic / instance inference."""
+    _padding_and_resize(cuda, pad=(160, 192), img=(150, 171), outsz=(97, 111))
+
+
+def test_postprocess_with_padding_and_resize_portrait(cuda):
+    """the same in portrait: padded input 192 x 160, image 171 x 150, output 111 x 97"""
+    _padding_and_resize(cuda, pad=(192, 160), img=(171, 150), outsz=(111, 97))
+
+
+def _padding_and_resize(cuda, pad, img, outsz):
     from odise_b200.postprocess import PostProcessor
     from oracle import postprocess as opp
-    B, Q, K, h, w = 1, 30, 11, 40, 48                       # padded input 160 x 192, image 150 x 171, output 97 x 111
-    pad, img, outsz = (160, 192), (150, 171), (97, 111)
+    B, Q, K, h, w = 1, 30, 11, pad[0] // 4, pad[1] // 4
     cls, masks = _case(9, B, Q, K, h, w)
     things = list(range(0, K, 2))
     pp = PostProcessor(cuda, K, things)
