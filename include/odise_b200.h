@@ -467,6 +467,76 @@ int odise_masked_xattn_backward_bf16(const void* q, const void* k, const void* v
                                      void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Mask2Former SetCriterion for training (matcher.py:15-156, criterion.py:21-197): Hungarian matching costs and the
+ * point-sampled mask losses with their backward.  pred [B, Q, H, W] in float, __half or __nv_bfloat16 (_f32 / _f16 /
+ * _bf16); target masks tgt [sum T, Hg, Wg] bytes (0 / 1: a torch bool or uint8 tensor), image b's targets first-to-last
+ * after those of images 0..b-1.  Points are float32 (x, y) in [0, 1)^2, sampled as detectron2's point_sample does
+ * (grid_sample, bilinear, zeros padding, align_corners=False) with the fp32 roundings of torch's CUDA kernel, so every
+ * sampled logit is bit-equal to torch's on the float32 upcast of pred.  All arithmetic is fp32.
+ *
+ * odise_mask_cost_*: cost [B, Q, Tmax] float32 (columns t >= T_b not written) of one prediction set,
+ *   C[b, q, t] = w_mask * CE + w_class * (-prob[b, q, labels[t]]) + w_dice * dice over the P points[b] [B, P, 2] of
+ *   image b, CE = mean_p softplus(-x) t + softplus(x) (1 - t), dice = 1 - (2 sum sigma(x) t + 1) / (sum sigma(x) + sum t
+ *   + 1).  prob [B, Q, K1] float32, labels [sum T] int64 (a label outside [0, K1) gives NaN), tgt_counts: T_b of each
+ *   image in HOST memory (B <= ODISE_MASK_MAX_IMAGES, T_b <= Tmax).
+ * odise_mask_loss_forward_*: the mask losses of N matched pairs, pairs [N, 3] int64 = (b, q, global target index), in
+ *   the order the loss sums them.  Pair n samples its S candidates cand [N, S, 2], keeps the k with the smallest |logit|
+ *   (exact ties: lowest candidate index) and appends the P - k random points rnd [N, P - k, 2]; losses [2] float32 =
+ *   (sum_n mean_p BCE / num_masks, sum_n dice_n / num_masks).  S <= ODISE_MASK_MAX_CANDIDATES, P <=
+ *   ODISE_MASK_MAX_POINTS, k <= min(P, S) (ODISE_ERR_UNSUPPORTED / ODISE_ERR_ARG otherwise).  The workspace
+ *   (odise_mask_loss_workspace_bytes(N, P), 16-byte aligned) receives the state the backward reads: per-pair sums
+ *   [N, 4] float32, then the pairs' P loss points [N, P, 2] float32 (the selected candidates in candidate order, then the
+ *   random points).
+ * odise_mask_loss_backward_*: grad_pred [B, Q, H, W] in pred's type, every element written (0 for queries that
+ *   pair_of [B*Q] int64 maps to -1, else to their pair), from grad_losses [2] float32 on the device.  Summed in int64
+ *   fixed point, so bit-reproducible; rounded once from the fixed-point sum.
+ * odise_mask_point_sample_*: out [N, P] float32 = the samples of maps [N, H, W] (_u8: bytes) at points [N, P, 2],
+ *   as the kernels above take them: detectron2's point_sample on the device.
+ * Every result is reduced in a fixed order.  No host synchronisation and no allocation. */
+#define ODISE_MASK_MAX_IMAGES 256
+#define ODISE_MASK_MAX_CANDIDATES 53248
+#define ODISE_MASK_MAX_POINTS 32768
+long long odise_mask_loss_workspace_bytes(int N, int P);
+int odise_mask_cost_f32(const void* pred, const float* prob, const long long* labels, const uint8_t* tgt,
+                        const float* points, const int* tgt_counts, float* cost, int B, int Q, int H, int W, int K1,
+                        int Hg, int Wg, int Tmax, int P, float w_class, float w_mask, float w_dice, void* stream);
+int odise_mask_cost_f16(const void* pred, const float* prob, const long long* labels, const uint8_t* tgt,
+                        const float* points, const int* tgt_counts, float* cost, int B, int Q, int H, int W, int K1,
+                        int Hg, int Wg, int Tmax, int P, float w_class, float w_mask, float w_dice, void* stream);
+int odise_mask_cost_bf16(const void* pred, const float* prob, const long long* labels, const uint8_t* tgt,
+                         const float* points, const int* tgt_counts, float* cost, int B, int Q, int H, int W, int K1,
+                         int Hg, int Wg, int Tmax, int P, float w_class, float w_mask, float w_dice, void* stream);
+int odise_mask_point_sample_f32(const void* maps, const float* points, float* out, int N, int H, int W, int P,
+                                void* stream);
+int odise_mask_point_sample_f16(const void* maps, const float* points, float* out, int N, int H, int W, int P,
+                                void* stream);
+int odise_mask_point_sample_bf16(const void* maps, const float* points, float* out, int N, int H, int W, int P,
+                                 void* stream);
+int odise_mask_point_sample_u8(const void* maps, const float* points, float* out, int N, int H, int W, int P,
+                               void* stream);
+int odise_mask_loss_forward_f32(const void* pred, const uint8_t* tgt, const long long* pairs, const float* cand,
+                                const float* rnd, void* workspace, float* losses, int B, int Q, int H, int W, int Hg,
+                                int Wg, int N, int P, int S, int k, float num_masks, void* stream);
+int odise_mask_loss_forward_f16(const void* pred, const uint8_t* tgt, const long long* pairs, const float* cand,
+                                const float* rnd, void* workspace, float* losses, int B, int Q, int H, int W, int Hg,
+                                int Wg, int N, int P, int S, int k, float num_masks, void* stream);
+int odise_mask_loss_forward_bf16(const void* pred, const uint8_t* tgt, const long long* pairs, const float* cand,
+                                 const float* rnd, void* workspace, float* losses, int B, int Q, int H, int W, int Hg,
+                                 int Wg, int N, int P, int S, int k, float num_masks, void* stream);
+int odise_mask_loss_backward_f32(const void* pred, const uint8_t* tgt, const long long* pairs,
+                                 const long long* pair_of, const void* workspace, const float* grad_losses,
+                                 void* grad_pred, int B, int Q, int H, int W, int Hg, int Wg, int N, int P,
+                                 float num_masks, void* stream);
+int odise_mask_loss_backward_f16(const void* pred, const uint8_t* tgt, const long long* pairs,
+                                 const long long* pair_of, const void* workspace, const float* grad_losses,
+                                 void* grad_pred, int B, int Q, int H, int W, int Hg, int Wg, int N, int P,
+                                 float num_masks, void* stream);
+int odise_mask_loss_backward_bf16(const void* pred, const uint8_t* tgt, const long long* pairs,
+                                  const long long* pair_of, const void* workspace, const float* grad_losses,
+                                  void* grad_pred, int B, int Q, int H, int W, int Hg, int Wg, int N, int P,
+                                  float num_masks, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

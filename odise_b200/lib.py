@@ -79,6 +79,20 @@ _SIGS = {
     "odise_masked_xattn_backward_f32": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
     "odise_masked_xattn_backward_f16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
     "odise_masked_xattn_backward_bf16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
+    "odise_mask_loss_workspace_bytes": [c_int] * 2,          # returns long long (set in load())
+    "odise_mask_cost_f32": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
+    "odise_mask_cost_f16": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
+    "odise_mask_cost_bf16": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
+    "odise_mask_point_sample_f32": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
+    "odise_mask_point_sample_f16": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
+    "odise_mask_point_sample_bf16": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
+    "odise_mask_point_sample_u8": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
+    "odise_mask_loss_forward_f32": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
+    "odise_mask_loss_forward_f16": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
+    "odise_mask_loss_forward_bf16": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
+    "odise_mask_loss_backward_f32": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
+    "odise_mask_loss_backward_f16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
+    "odise_mask_loss_backward_bf16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -189,6 +203,7 @@ def load():
         fn.restype = c_int
     lib.odise_msda_det_workspace_bytes.restype = c_longlong
     lib.odise_masked_xattn_workspace_bytes.restype = c_longlong
+    lib.odise_mask_loss_workspace_bytes.restype = c_longlong
     _lib = lib
     return lib
 
@@ -811,6 +826,144 @@ def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
     _check(getattr(load(), fn)(_ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out), _ptr(lse), _ptr(grad_out),
                                _ptr(gq), _ptr(gk), _ptr(gv), B, heads, 32, Q, S, _ptr(ws), _stream()), fn)
     return gq, gk, gv
+
+
+MASK_MAX_IMAGES, MASK_MAX_CANDIDATES, MASK_MAX_POINTS = 256, 53248, 32768    # ODISE_MASK_MAX_* of the header
+
+
+def _mask_maps(pred, tgt):
+    """Checks shared by the mask-criterion entry points: pred [B, Q, H, W] float32 / float16 / bfloat16 and the target
+    masks tgt [sum T, Hg, Wg] bool or uint8, both CUDA and contiguous.  -> (suffix, B, Q, H, W, Hg, Wg)"""
+    if pred.dtype not in _XATTN_SFX:
+        raise OdiseError(f"pred_masks: expected float32, float16 or bfloat16, got {pred.dtype}")
+    if tgt.dtype not in (torch.bool, torch.uint8):
+        raise OdiseError(f"target masks: expected bool or uint8, got {tgt.dtype}")
+    for t, nm in ((pred, "pred_masks"), (tgt, "target masks")):
+        if not t.is_cuda:
+            raise OdiseError(f"{nm} must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise OdiseError(f"{nm} tensor has to be contiguous")
+    if pred.dim() != 4 or tgt.dim() != 3:
+        raise OdiseError(f"pred_masks must be [B, Q, H, W] and target masks [T, Hg, Wg], got {tuple(pred.shape)} and "
+                         f"{tuple(tgt.shape)}")
+    B, Q, H, W = pred.shape
+    if min(B, Q, H, W) <= 0 or min(tgt.shape[1:]) <= 0:
+        raise OdiseError(f"empty maps: pred_masks {tuple(pred.shape)}, target masks {tuple(tgt.shape)}")
+    if B > MASK_MAX_IMAGES:
+        raise OdiseError(f"mask criterion: at most {MASK_MAX_IMAGES} images, got {B}")
+    return _XATTN_SFX[pred.dtype], B, Q, H, W, tgt.shape[1], tgt.shape[2]
+
+
+def _req_shape(t, dtype, shape, nm):
+    if not t.is_cuda or t.dtype != dtype or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+        raise OdiseError(f"{nm}: expected a contiguous CUDA {dtype} tensor of shape {tuple(shape)}, got "
+                         f"{t.dtype} {tuple(t.shape)} on {t.device}")
+
+
+def _u8(t):
+    return t.view(torch.uint8) if t.dtype == torch.bool else t
+
+
+def mask_point_sample(maps, points):
+    """detectron2's point_sample on the device, as the mask-criterion kernels sample (odise_mask_point_sample_*):
+    maps [N, H, W] float32 / float16 / bfloat16 / bool / uint8, points [N, P, 2] float32 in [0, 1)^2 -> [N, P] float32,
+    bit-equal to F.grid_sample(maps[:, None].float(), 2 * points[:, :, None] - 1, align_corners=False)."""
+    sfx = {torch.bool: "u8", torch.uint8: "u8"}.get(maps.dtype) or _XATTN_SFX.get(maps.dtype)
+    if sfx is None:
+        raise OdiseError(f"maps: expected float32, float16, bfloat16, bool or uint8, got {maps.dtype}")
+    if not maps.is_cuda or not maps.is_contiguous() or maps.dim() != 3:
+        raise OdiseError(f"maps: expected a contiguous CUDA tensor [N, H, W], got {tuple(maps.shape)} on {maps.device}")
+    N, H, W = maps.shape
+    if points.dim() != 3 or points.shape[0] != N or points.shape[2] != 2:
+        raise OdiseError(f"points: expected [{N}, P, 2], got {tuple(points.shape)}")
+    _req_shape(points, torch.float32, tuple(points.shape), "points")
+    out = torch.empty(N, points.shape[1], dtype=torch.float32, device=maps.device)
+    fn = "odise_mask_point_sample_" + sfx
+    _check(getattr(load(), fn)(_ptr(_u8(maps)), _ptr(points), _ptr(out), N, H, W, points.shape[1], _stream()), fn)
+    return out
+
+
+def mask_cost(pred, prob, labels, tgt, points, counts, w_class, w_mask, w_dice, out=None):
+    """Matching costs of one prediction set (odise_mask_cost_f32 / _f16 / _bf16 by pred.dtype): pred [B, Q, H, W],
+    prob [B, Q, K1] float32 (softmax of the class logits), labels [sum T] int64, tgt [sum T, Hg, Wg] bool / uint8 with
+    image b's counts[b] targets after those of images 0..b-1 (counts: a Python list), points [B, P, 2] float32 ->
+    cost [B, Q, max(counts)] float32 (out: a tensor of that shape and dtype to write into; columns t >= counts[b] are
+    left as they are).  OdiseError on CPU, non-contiguous or wrongly typed tensors and on shapes that disagree."""
+    sfx, B, Q, H, W, Hg, Wg = _mask_maps(pred, tgt)
+    counts = [int(c) for c in counts]
+    if len(counts) != B or min(counts, default=0) < 0 or sum(counts) != tgt.shape[0]:
+        raise OdiseError(f"target counts {counts} do not match {B} images and {tgt.shape[0]} target masks")
+    if prob.dim() != 3 or tuple(prob.shape[:2]) != (B, Q):
+        raise OdiseError(f"prob: expected [B, Q, K1] = [{B}, {Q}, K1], got {tuple(prob.shape)}")
+    K1 = prob.shape[2]
+    if points.dim() != 3 or points.shape[0] != B or points.shape[2] != 2 or points.shape[1] <= 0:
+        raise OdiseError(f"points: expected [{B}, P, 2] with P > 0, got {tuple(points.shape)}")
+    P = points.shape[1]
+    _req_shape(prob, torch.float32, (B, Q, K1), "prob")
+    _req_shape(labels, torch.int64, (tgt.shape[0],), "labels")
+    _req_shape(points, torch.float32, (B, P, 2), "points")
+    Tmax = max(counts, default=0)
+    if out is None:
+        out = torch.empty(B, Q, Tmax, dtype=torch.float32, device=pred.device)
+    _req_shape(out, torch.float32, (B, Q, Tmax), "out")
+    cnt = (ctypes.c_int * B)(*counts)
+    fn = "odise_mask_cost_" + sfx
+    _check(getattr(load(), fn)(_ptr(pred), _ptr(prob), _ptr(labels), _ptr(_u8(tgt)), _ptr(points), cnt, _ptr(out),
+                               B, Q, H, W, K1, Hg, Wg, Tmax, P, float(w_class), float(w_mask), float(w_dice),
+                               _stream()), fn)
+    return out
+
+
+def _mask_loss_shapes(pred, tgt, pairs, num_points):
+    """Checks shared by the mask-loss entry points: pairs [N, 3] int64 and 0 < num_points <= MASK_MAX_POINTS.
+    -> (suffix, B, Q, H, W, Hg, Wg, N)"""
+    sfx, B, Q, H, W, Hg, Wg = _mask_maps(pred, tgt)
+    if pairs.dim() != 2 or pairs.shape[1] != 3:
+        raise OdiseError(f"pairs must be [N, 3], got {tuple(pairs.shape)}")
+    _req_shape(pairs, torch.int64, tuple(pairs.shape), "pairs")
+    if not 0 < num_points <= MASK_MAX_POINTS:
+        raise OdiseError(f"mask loss: num_points = {num_points} not supported (1 .. {MASK_MAX_POINTS})")
+    return sfx, B, Q, H, W, Hg, Wg, pairs.shape[0]
+
+
+def mask_loss_forward(pred, tgt, pairs, cand, rnd, num_masks, num_points, k):
+    """Point-sampled mask losses of N matched pairs (odise_mask_loss_forward_* by pred.dtype): pairs [N, 3] int64 =
+    (image, query, row of tgt), cand [N, S, 2] the oversampled candidates, of which the k with the smallest |logit| are
+    kept, rnd [N, num_points - k, 2] the random points -> (losses [2] float32 = (loss_mask, loss_dice), state): state is
+    the workspace the backward reads: sums [N, 4] float32, then the P loss points of each pair [N, P, 2] float32 (the
+    selected candidates in candidate order, then the random points)."""
+    sfx, B, Q, H, W, Hg, Wg, N = _mask_loss_shapes(pred, tgt, pairs, num_points)
+    if cand.dim() != 3:
+        raise OdiseError(f"cand must be [N, S, 2], got {tuple(cand.shape)}")
+    S = cand.shape[1]
+    if not (S <= MASK_MAX_CANDIDATES and 0 <= k <= min(num_points, S)):
+        raise OdiseError(f"mask loss: {S} candidates, k = {k} not supported (candidates <= {MASK_MAX_CANDIDATES}, "
+                         f"k <= min(num_points, candidates))")
+    _req_shape(cand, torch.float32, (N, S, 2), "cand")
+    _req_shape(rnd, torch.float32, (N, num_points - k, 2), "rnd")
+    ws = torch.empty(max(int(load().odise_mask_loss_workspace_bytes(N, num_points)), 16), dtype=torch.uint8,
+                     device=pred.device)
+    losses = torch.empty(2, dtype=torch.float32, device=pred.device)
+    fn = "odise_mask_loss_forward_" + sfx
+    _check(getattr(load(), fn)(_ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(cand), _ptr(rnd), _ptr(ws), _ptr(losses),
+                               B, Q, H, W, Hg, Wg, N, num_points, S, k, float(num_masks), _stream()), fn)
+    return losses, ws
+
+
+def mask_loss_backward(pred, tgt, pairs, pair_of, state, grad_losses, num_masks, num_points):
+    """Backward of mask_loss_forward (odise_mask_loss_backward_*): state as it returned, grad_losses [2] float32 on the
+    device -> grad_pred shaped and typed like pred, zero on the queries pair_of [B*Q] int64 maps to -1.
+    Bit-reproducible (int64 fixed-point sums)."""
+    sfx, B, Q, H, W, Hg, Wg, N = _mask_loss_shapes(pred, tgt, pairs, num_points)
+    _req_shape(pair_of, torch.int64, (B * Q,), "pair_of")
+    _req_shape(grad_losses, torch.float32, (2,), "grad_losses")
+    if not state.is_cuda or state.dtype != torch.uint8 or state.numel() < N * (16 + 8 * num_points):
+        raise OdiseError("state: expected the workspace mask_loss_forward returned")
+    grad = torch.empty_like(pred)
+    fn = "odise_mask_loss_backward_" + sfx
+    _check(getattr(load(), fn)(_ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(pair_of), _ptr(state), _ptr(grad_losses),
+                               _ptr(grad), B, Q, H, W, Hg, Wg, N, num_points, float(num_masks), _stream()), fn)
+    return grad
 
 
 class nvtx:
