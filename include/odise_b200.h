@@ -537,6 +537,53 @@ int odise_mask_loss_backward_bf16(const void* pred, const uint8_t* tgt, const lo
                                   float num_masks, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Decoder prediction heads for training (odise.py:729-776 forward_prediction_heads with PooledMaskEmbed / MaskPooling,
+ * :923-1015, hard pooling): mask_embed E [B, Q, C], mask_features X [B, C, H, W], all contiguous, C = 256 and
+ * Q <= 256 (ODISE_ERR_UNSUPPORTED otherwise), H * W < 2^24.  _f32 / _f16 / _bf16: every tensor but weights in float,
+ * __half or __nv_bfloat16; all arithmetic fp32, every output rounded once.
+ * odise_mask_head_forward_*: outputs_mask [B, Q, H, W] = E X; the hard mask m = sigmoid(outputs_mask as stored) >
+ *   threshold (sigmoid in fp32 rounded to the storage type, compared in fp32); weights [B, Q] float32 = w =
+ *   T(1 / (sum m + 1e-8)), 0 for an empty mask; pooled [B, Q, C] = T(w * sum_hw m X) (a zero row for an empty mask).
+ * odise_mask_head_backward_*: from the forward's inputs, its outputs_mask and weights, grad_mask [B, Q, H, W] and
+ *   grad_pooled [B, Q, C]: grad_embed [B, Q, C] = grad_mask X^T and grad_features [B, C, H, W] = E^T grad_mask +
+ *   (grad_pooled o w)^T m, with m recomputed from outputs_mask.
+ * The workspace (odise_mask_head_workspace_bytes(B, Q, C, H, W) bytes, 16-byte aligned, any content; 0 for shapes the
+ *   entry points refuse) holds fp32 split partials; their split counts depend on the shape only and they are summed in
+ *   split order, without atomics, so every result is bit-reproducible.
+ * odise_mask_head_attn_mask_*: attn_mask [B*heads, Q, h*w] bytes (a torch bool tensor, 1 = blocked) = sigmoid(bilinear
+ *   resize of outputs_mask [B, Q, H, W] to h x w, align_corners=False) < 0.5, each value rounded to the storage type as
+ *   torch's ops round it, written for every head; a row whose keys are all blocked is written all 0 (odise.py:683).
+ * No host synchronisation and no allocation (CUDA-graph capturable). */
+long long odise_mask_head_workspace_bytes(int B, int Q, int C, int H, int W);
+int odise_mask_head_forward_f32(const void* mask_embed, const void* mask_features, void* outputs_mask, void* pooled,
+                                float* weights, int B, int Q, int C, int H, int W, float threshold, void* workspace,
+                                void* stream);
+int odise_mask_head_forward_f16(const void* mask_embed, const void* mask_features, void* outputs_mask, void* pooled,
+                                float* weights, int B, int Q, int C, int H, int W, float threshold, void* workspace,
+                                void* stream);
+int odise_mask_head_forward_bf16(const void* mask_embed, const void* mask_features, void* outputs_mask, void* pooled,
+                                 float* weights, int B, int Q, int C, int H, int W, float threshold, void* workspace,
+                                 void* stream);
+int odise_mask_head_attn_mask_f32(const void* outputs_mask, uint8_t* attn_mask, int B, int Q, int H, int W, int h,
+                                  int w, int heads, void* stream);
+int odise_mask_head_attn_mask_f16(const void* outputs_mask, uint8_t* attn_mask, int B, int Q, int H, int W, int h,
+                                  int w, int heads, void* stream);
+int odise_mask_head_attn_mask_bf16(const void* outputs_mask, uint8_t* attn_mask, int B, int Q, int H, int W, int h,
+                                   int w, int heads, void* stream);
+int odise_mask_head_backward_f32(const void* mask_embed, const void* mask_features, const void* outputs_mask,
+                                 const float* weights, const void* grad_mask, const void* grad_pooled, void* grad_embed,
+                                 void* grad_features, int B, int Q, int C, int H, int W, float threshold,
+                                 void* workspace, void* stream);
+int odise_mask_head_backward_f16(const void* mask_embed, const void* mask_features, const void* outputs_mask,
+                                 const float* weights, const void* grad_mask, const void* grad_pooled, void* grad_embed,
+                                 void* grad_features, int B, int Q, int C, int H, int W, float threshold,
+                                 void* workspace, void* stream);
+int odise_mask_head_backward_bf16(const void* mask_embed, const void* mask_features, const void* outputs_mask,
+                                  const float* weights, const void* grad_mask, const void* grad_pooled,
+                                  void* grad_embed, void* grad_features, int B, int Q, int C, int H, int W,
+                                  float threshold, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

@@ -12,6 +12,7 @@
 #include "ptx.cuh"
 #include "odise_b200.h"
 #include "launch_count.h"
+#include "mask_resize.cuh"
 
 namespace ob {
 
@@ -42,15 +43,7 @@ attn_mask_bits_kernel(const float* __restrict__ logits, uint32_t* __restrict__ b
     bool allowed = false;
     if (key < HW) {
       const int oy = key / Wl, ox = key - oy * Wl;
-      // F.interpolate(bilinear, align_corners=False) source index (ATen area_pixel_compute_source_index)
-      const float fy = fmaxf((oy + 0.5f) * sy - 0.5f, 0.f), fx = fmaxf((ox + 0.5f) * sx - 0.5f, 0.f);
-      const int y0 = (int)fy, x0 = (int)fx;
-      const int y1 = y0 + (y0 < Hm - 1 ? 1 : 0), x1 = x0 + (x0 < Wm - 1 ? 1 : 0);
-      const float ly = fy - y0, lx = fx - x0, hy = 1.f - ly, hx = 1.f - lx;
-      const float v = hy * (hx * src[y0 * Wm + x0] + lx * src[y0 * Wm + x1]) +
-                      ly * (hx * src[y1 * Wm + x0] + lx * src[y1 * Wm + x1]);
-      const float s = 1.f / (1.f + expf(-v));
-      allowed = !(s < 0.5f);  // attn_mask = sigmoid(.) < 0.5 means "blocked"
+      allowed = !mr_blocked(src, Hm, Wm, oy, ox, sy, sx);  // attn_mask = sigmoid(.) < 0.5 means "blocked"
     }
     const uint32_t w = __ballot_sync(0xffffffffu, allowed);
     if ((threadIdx.x & 31) == 0) dst[base >> 5] = w;

@@ -93,6 +93,16 @@ _SIGS = {
     "odise_mask_loss_backward_f32": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
     "odise_mask_loss_backward_f16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
     "odise_mask_loss_backward_bf16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
+    "odise_mask_head_workspace_bytes": [c_int] * 5,          # returns long long (set in load())
+    "odise_mask_head_forward_f32": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_mask_head_forward_f16": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_mask_head_forward_bf16": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_mask_head_attn_mask_f32": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
+    "odise_mask_head_attn_mask_f16": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
+    "odise_mask_head_attn_mask_bf16": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
+    "odise_mask_head_backward_f32": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_mask_head_backward_f16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_mask_head_backward_bf16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -204,6 +214,7 @@ def load():
     lib.odise_msda_det_workspace_bytes.restype = c_longlong
     lib.odise_masked_xattn_workspace_bytes.restype = c_longlong
     lib.odise_mask_loss_workspace_bytes.restype = c_longlong
+    lib.odise_mask_head_workspace_bytes.restype = c_longlong
     _lib = lib
     return lib
 
@@ -964,6 +975,99 @@ def mask_loss_backward(pred, tgt, pairs, pair_of, state, grad_losses, num_masks,
     _check(getattr(load(), fn)(_ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(pair_of), _ptr(state), _ptr(grad_losses),
                                _ptr(grad), B, Q, H, W, Hg, Wg, N, num_points, float(num_masks), _stream()), fn)
     return grad
+
+
+MASK_HEAD_C, MASK_HEAD_MAX_Q = 256, 256    # the mask width and query count the mask-head kernels take
+
+
+def _mask_head_shapes(embed, features, outputs_mask=None, weights=None, grad_mask=None, grad_pooled=None):
+    """Checks of the mask-head entry points, without data and without the library (the fake implementations of
+    odise_b200.decoder's ops call it too): embed [B, Q, 256] and features [B, 256, H, W] contiguous CUDA tensors of one
+    dtype of float32 / float16 / bfloat16, Q <= 256, H * W < 2^24; for the backward outputs_mask and grad_mask
+    [B, Q, H, W] and grad_pooled [B, Q, 256] of that dtype and weights [B, Q] float32.  -> (suffix, B, Q, H, W)"""
+    if embed.dtype not in _XATTN_SFX:
+        raise OdiseError(f"mask_embed: expected float32, float16 or bfloat16, got {embed.dtype}")
+    if embed.dim() != 3 or features.dim() != 4:
+        raise OdiseError(f"mask_embed must be [B, Q, C] and mask_features [B, C, H, W], got {tuple(embed.shape)} and "
+                         f"{tuple(features.shape)}")
+    B, Q, C = embed.shape
+    H, W = features.shape[2:]
+    if C != MASK_HEAD_C or not 0 < Q <= MASK_HEAD_MAX_Q:
+        raise OdiseError(f"mask head: C = {C}, Q = {Q} not supported (C = {MASK_HEAD_C}, Q <= {MASK_HEAD_MAX_Q})")
+    if min(B, H, W) <= 0 or H * W >= 2 ** 24 or B > 65535:
+        raise OdiseError(f"mask head: B = {B}, H x W = {H} x {W} not supported (B <= 65535, 0 < H*W < 2^24)")
+    want = {"mask_features": (B, C, H, W), "outputs_mask": (B, Q, H, W), "grad_mask": (B, Q, H, W),
+            "grad_pooled": (B, Q, C)}
+    for t, nm in ((embed, "mask_embed"), (features, "mask_features"), (outputs_mask, "outputs_mask"),
+                  (grad_mask, "grad_mask"), (grad_pooled, "grad_pooled")):
+        if t is not None:
+            _req_shape(t, embed.dtype, want.get(nm, tuple(embed.shape)), nm)
+    if weights is not None:
+        _req_shape(weights, torch.float32, (B, Q), "weights")
+    return _XATTN_SFX[embed.dtype], B, Q, H, W
+
+
+def _mask_head_workspace(B, Q, H, W, device):
+    """workspace of the mask-head entry points (odise_mask_head_workspace_bytes), from torch's allocator"""
+    return torch.empty(int(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W)), dtype=torch.uint8,
+                       device=device)
+
+
+def mask_head_forward(embed, features, threshold=0.5):
+    """The prediction head's mask logits and hard mask pooling (odise_mask_head_forward_* by dtype): embed [B, Q, 256],
+    features [B, 256, H, W] -> (outputs_mask [B, Q, H, W], pooled [B, Q, 256], both in embed's dtype, weights [B, Q]
+    float32 = the per-(b, q) factor 1 / (count + 1e-8) as the pooling applied it).  OdiseError on CPU, non-contiguous or
+    mixed-dtype tensors and on shapes the kernels do not take."""
+    sfx, B, Q, H, W = _mask_head_shapes(embed, features)
+    om = torch.empty(B, Q, H, W, dtype=embed.dtype, device=embed.device)
+    pooled = torch.empty_like(embed)
+    weights = torch.empty(B, Q, dtype=torch.float32, device=embed.device)
+    ws = _mask_head_workspace(B, Q, H, W, embed.device)
+    fn = "odise_mask_head_forward_" + sfx
+    _check(getattr(load(), fn)(_ptr(embed), _ptr(features), _ptr(om), _ptr(pooled), _ptr(weights), B, Q, MASK_HEAD_C,
+                               H, W, float(threshold), _ptr(ws), _stream()), fn)
+    return om, pooled, weights
+
+
+def _mask_head_attn_shapes(outputs_mask, size, heads):
+    """Checks of mask_head_attn_mask (shared with its fake): -> (suffix, B, Q, H, W, h, w)"""
+    if outputs_mask.dtype not in _XATTN_SFX:
+        raise OdiseError(f"outputs_mask: expected float32, float16 or bfloat16, got {outputs_mask.dtype}")
+    if outputs_mask.dim() != 4:
+        raise OdiseError(f"outputs_mask must be [B, Q, H, W], got {tuple(outputs_mask.shape)}")
+    _req_shape(outputs_mask, outputs_mask.dtype, tuple(outputs_mask.shape), "outputs_mask")
+    B, Q, H, W = outputs_mask.shape
+    h, w = (int(s) for s in size)
+    if min(B, Q, H, W, h, w, heads) <= 0 or B * Q >= 2 ** 31 or h * w >= 2 ** 31:
+        raise OdiseError(f"attention mask: outputs_mask {tuple(outputs_mask.shape)}, size {(h, w)}, heads {heads} not "
+                         "supported")
+    return _XATTN_SFX[outputs_mask.dtype], B, Q, H, W, h, w
+
+
+def mask_head_attn_mask(outputs_mask, size, heads):
+    """The decoder's attention mask (odise_mask_head_attn_mask_*): outputs_mask [B, Q, H, W] -> bool
+    [B*heads, Q, h*w], True = blocked = sigmoid(bilinear resize to size = (h, w)) < 0.5 in torch's roundings for the
+    dtype, with every all-blocked row written all False (odise.py:683)."""
+    sfx, B, Q, H, W, h, w = _mask_head_attn_shapes(outputs_mask, size, heads)
+    out = torch.empty(B * heads, Q, h * w, dtype=torch.bool, device=outputs_mask.device)
+    fn = "odise_mask_head_attn_mask_" + sfx
+    _check(getattr(load(), fn)(_ptr(outputs_mask), _ptr(out), B, Q, H, W, h, w, heads, _stream()), fn)
+    return out
+
+
+def mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_pooled, threshold=0.5):
+    """Backward of mask_head_forward (odise_mask_head_backward_*) -> (grad_embed, grad_features) in embed's dtype:
+    grad_mask X^T and E^T grad_mask + (grad_pooled o weights)^T m, m the hard mask of outputs_mask.  Bit-reproducible
+    (fixed-order sums, no atomics).  Errors as mask_head_forward, and for the saved tensors or gradients of the wrong
+    shape or dtype."""
+    sfx, B, Q, H, W = _mask_head_shapes(embed, features, outputs_mask, weights, grad_mask, grad_pooled)
+    ge, gx = torch.empty_like(embed), torch.empty_like(features)
+    ws = _mask_head_workspace(B, Q, H, W, embed.device)
+    fn = "odise_mask_head_backward_" + sfx
+    _check(getattr(load(), fn)(_ptr(embed), _ptr(features), _ptr(outputs_mask), _ptr(weights), _ptr(grad_mask),
+                               _ptr(grad_pooled), _ptr(ge), _ptr(gx), B, Q, MASK_HEAD_C, H, W, float(threshold),
+                               _ptr(ws), _stream()), fn)
+    return ge, gx
 
 
 class nvtx:
