@@ -294,3 +294,72 @@ def test_gemm_tma_store_epilogue(cuda, kind, cfg):
         tol = 1e-4 if kind != "planes_hi_only" else 6e-3
         assert _rel(got[:, :, pad:pad + N], ref) < tol
         assert (got[:, :, :pad] == 0).all() and (got[:, :, pad + N:N + 2 * pad] == 0).all()
+
+
+@pytest.mark.parametrize("nmma", [3, 1])
+@pytest.mark.parametrize("bn", [0, 64, 128, 256])
+@pytest.mark.parametrize("case", ["unet", "clip", "clip_hi_only", "decoder", "vae_bf16", "clip_split_k"])
+def test_gemm_vt_producer(cuda, record, nmma, bn, case):
+    """The attention kernels' V^T operand, written by the swapped-operand GEMM V^T = W X^T + bias_m[:, None] into
+    (hi, lo) planes: fp16 pairs for odise_attention_tc (clip.py:56, head.py:338, unet.py:212), bf16 pairs for the VAE's
+    P V GEMM (vae.py:126).  unet: M = heads * HS with zero pad rows in W, no bias_m | clip: M = 1024, N = B * 584 |
+    decoder: batch = B over image row blocks of the level memory (b_bs), image z written at column z * hw8, N = hw = 252,
+    whose 4 pad columns per image must stay untouched | clip_split_k: bias_m applied by the split-K reduce kernel.
+    Ragged N and forced tile widths send tiles through both the interior epilogue and epilogue_quad."""
+    from odise_b200 import lib, ops
+    g = torch.Generator().manual_seed(len(case) * 13 + bn + nmma)
+    f16, lo, batch, split_k = True, True, 1, 1
+    if case == "unet":
+        heads, d, HS, C, N = 8, 40, 64, 320, 2 * 1024
+        W = ops.head_pad_rows(torch.randn(heads * d, C, generator=g) * C ** -0.5, heads, d, HS)
+        bm = None
+    elif case == "decoder":
+        B, S, start, hw, hw8, C = 2, 400, 100, 252, 256, 256
+        W = torch.randn(3 * 8 * 64, C, generator=g) * C ** -0.5
+        bm = torch.randn(W.shape[0], generator=g)
+        N, batch = hw, B
+    else:
+        C, B, TS = 1024, 2, 584
+        if case == "vae_bf16":
+            C, B, TS = 512, 1, 4096
+        W = torch.randn(C, C, generator=g) * C ** -0.5
+        bm = torch.randn(C, generator=g)
+        N = B * TS
+        f16 = case != "vae_bf16"
+        lo = case != "clip_hi_only"
+        split_k = 4 if case == "clip_split_k" else 1
+    M = W.shape[0]
+    Wp = lib.split(W.to(cuda))
+    kw = dict(nmma=nmma, force_bn=bn, bias_m=None if bm is None else bm.to(cuda))
+    if split_k > 1:
+        kw.update(split_k=split_k, workspace=torch.empty(split_k * M * N, device=cuda))
+    if case == "decoder":
+        mem = torch.randn(B, S, C, generator=g)                  # level rows [start, start + hw) of every image
+        X = mem[:, start:start + hw]
+        xp = lib.split(mem.view(B * S, C).to(cuda)).row_slice(start, hw)
+        out = lib.Planes.empty(M, B * hw8, cuda, lo=lo, f16=f16)
+        kw.update(N=hw, batch=B, b_bs=S * xp.ld, outp_bs=hw8)
+        ref = torch.einsum("mc,btc->mbt", W.double(), X.double())
+    else:
+        X = torch.randn(N, C, generator=g)
+        xp = lib.split(X.to(cuda))
+        out = lib.Planes.empty(M, N, cuda, lo=lo, f16=f16)
+        ref = W.double() @ X.double().T
+    if bm is not None:
+        ref = ref + (bm.double().view(-1, 1, 1) if case == "decoder" else bm.double().view(-1, 1))
+    for t in (out.hi, out.lo):
+        if t is not None:
+            t.view(torch.int16).fill_(0x3C01)                   # a sentinel: 1.0009765625 in fp16, 1.0078125 in bf16
+    lib.gemm(Wp, xp, out_planes=out, **kw)
+    torch.cuda.synchronize()
+    got = out.float().cpu()
+    if case == "decoder":
+        got = got.view(M, B, hw8)
+        for t in (out.hi, out.lo):
+            if t is not None:
+                assert (t.view(torch.int16).view(M, B, hw8)[:, :, hw:] == 0x3C01).all()   # pad keys untouched
+        got = got[:, :, :hw]
+    tol = TOL[nmma] if lo else max(TOL[nmma], 1e-3 if f16 else 6e-3)   # hi only: one fp16 / bf16 rounding of the output
+    e = _rel(got, ref)
+    record(f"gemm V^T {case} bn={bn} nmma={nmma}: rel err {e:.3e}")
+    assert e < tol
