@@ -584,6 +584,24 @@ int odise_mask_head_backward_bf16(const void* mask_embed, const void* mask_featu
                                   float threshold, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * The pixel decoder's FPN step for training (msdeformattn.py:349), float32:
+ * odise_fpn_upsample_add_f32: y [N, C, H, W] = cur [N, C, H, W] + bilinear resize (align_corners=False) of the level
+ *   z to H x W, z read token-major: element (n, c, y, x) of the [N, C, h, w] level at z[n * z_batch_stride +
+ *   (y * w + x) * C + c] (a slice of the encoder's [N, S, C] memory, z_batch_stride >= h*w*C).  cur and y contiguous.
+ *   Bit-equal to torch's cur + F.interpolate(level, (H, W), "bilinear", align_corners=False) on CUDA for the
+ *   level's NCHW view of that memory, at every N: torch resizes that view with its NHWC frame kernel for N >= 2 and its
+ *   NCHW frame kernel for N = 1, which round the top row differently, and the kernel follows N.
+ * odise_fpn_upsample_add_backward_f32: grad_z = the adjoint of that resize applied to grad_y [N, C, H, W]
+ *   (contiguous), written token-major at grad_z[n * grad_z_batch_stride + (y * w + x) * C + c].  A gather over each
+ *   source element's outputs in a fixed order, no atomics: bit-reproducible.  The gradient of cur is grad_y.
+ * C a multiple of 32, N * C / 32 <= 65535, H, h <= 65535, h*w*C < 2^31 (ODISE_ERR_UNSUPPORTED otherwise).  No host
+ * synchronisation, no allocation, no workspace (CUDA-graph capturable). */
+int odise_fpn_upsample_add_f32(const float* z, long long z_batch_stride, const float* cur, float* y, int N, int C,
+                               int h, int w, int H, int W, void* stream);
+int odise_fpn_upsample_add_backward_f32(const float* grad_y, float* grad_z, long long grad_z_batch_stride, int N,
+                                        int C, int h, int w, int H, int W, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

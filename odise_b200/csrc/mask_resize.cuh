@@ -38,20 +38,44 @@ __device__ __forceinline__ float mr_sigmoid(float x) {
   return mr_round(1.f / (1.f + expf(-x)), static_cast<T*>(nullptr));
 }
 
+// one axis of torch's bilinear source coordinate for output index o, s = in / out in fp32 (area_pixel_compute_source_index
+// and the frame kernels): i0 = trunc(max(s * (o + 0.5) - 0.5, 0)), i1 = i0 + 1 unless i0 is the last of n sources,
+// l = the weight of i1, h = 1 - l the weight of i0.  The forward value (mr_bilinear) and the FPN backward's adjoint
+// weights and membership (fpn_upsample.cu) both come from here, so they agree bit for bit.
+struct MrAxis {
+  int i0, i1;
+  float h, l;
+};
+
+__device__ __forceinline__ MrAxis mr_axis(int o, float s, int n) {
+  const float f = fmaxf(__fmaf_rn(__fadd_rn((float)o, 0.5f), s, -0.5f), 0.f);
+  MrAxis a;
+  a.i0 = (int)f;
+  a.i1 = a.i0 + (a.i0 < n - 1 ? 1 : 0);
+  a.l = __fsub_rn(f, (float)a.i0);
+  a.h = __fsub_rn(1.f, a.l);
+  return a;
+}
+
+// torch's fp32 bilinear value at (ay, ax) of a source [Hm, Wm] whose element (y, x) is src[(y * Wm + x) * es].
+// top_ha selects the contraction of the top row: false fma(l, b, h * a), as in the NHWC frame kernel
+// (upsample_bilinear2d_nhwc_out_frame) and the bits of attn_mask_bits_kernel; true fma(h, a, l * b), as in
+// upsample_bilinear2d_out_frame where torch runs it for a batch-1 level view (measured on torch 2.11's sm_90 build).
+template <typename T, bool top_ha = false>
+__device__ __forceinline__ float mr_bilinear(const T* __restrict__ src, int Wm, const MrAxis& ay, const MrAxis& ax,
+                                             int es) {
+  const float a = mr_load(src + (ay.i0 * Wm + ax.i0) * es), b = mr_load(src + (ay.i0 * Wm + ax.i1) * es);
+  const float c = mr_load(src + (ay.i1 * Wm + ax.i0) * es), d = mr_load(src + (ay.i1 * Wm + ax.i1) * es);
+  const float top = top_ha ? __fmaf_rn(ax.h, a, __fmul_rn(ax.l, b)) : __fmaf_rn(ax.l, b, __fmul_rn(ax.h, a));
+  const float bot = __fmaf_rn(ax.h, c, __fmul_rn(ax.l, d));
+  return __fmaf_rn(ay.h, top, __fmul_rn(ay.l, bot));
+}
+
 // key (oy, ox) of the (Hl, Wl) level resized from src [Hm, Wm]; sy = Hm / Hl, sx = Wm / Wl in fp32
 template <typename T>
 __device__ __forceinline__ bool mr_blocked(const T* __restrict__ src, int Hm, int Wm, int oy, int ox, float sy,
                                            float sx) {
-  const float fy = fmaxf(__fmaf_rn(__fadd_rn((float)oy, 0.5f), sy, -0.5f), 0.f);
-  const float fx = fmaxf(__fmaf_rn(__fadd_rn((float)ox, 0.5f), sx, -0.5f), 0.f);
-  const int y0 = (int)fy, x0 = (int)fx;
-  const int y1 = y0 + (y0 < Hm - 1 ? 1 : 0), x1 = x0 + (x0 < Wm - 1 ? 1 : 0);
-  const float ly = __fsub_rn(fy, (float)y0), lx = __fsub_rn(fx, (float)x0);
-  const float hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
-  const float a = mr_load(src + y0 * Wm + x0), b = mr_load(src + y0 * Wm + x1);
-  const float c = mr_load(src + y1 * Wm + x0), d = mr_load(src + y1 * Wm + x1);
-  const float top = __fmaf_rn(lx, b, __fmul_rn(hx, a)), bot = __fmaf_rn(hx, c, __fmul_rn(lx, d));
-  const float v = __fmaf_rn(hy, top, __fmul_rn(ly, bot));
+  const float v = mr_bilinear(src, Wm, mr_axis(oy, sy, Hm), mr_axis(ox, sx, Wm), 1);
   return mr_sigmoid<T>(mr_round(v, static_cast<T*>(nullptr))) < 0.5f;
 }
 

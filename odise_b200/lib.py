@@ -103,6 +103,8 @@ _SIGS = {
     "odise_mask_head_backward_f32": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
     "odise_mask_head_backward_f16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
     "odise_mask_head_backward_bf16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
+    "odise_fpn_upsample_add_f32": [c_void_p, c_longlong, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p],
+    "odise_fpn_upsample_add_backward_f32": [c_void_p, c_void_p, c_longlong] + [c_int] * 6 + [c_void_p],
     "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
     "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
     "odise_profile_begin": [],
@@ -1068,6 +1070,74 @@ def mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_p
                                _ptr(grad_pooled), _ptr(ge), _ptr(gx), B, Q, MASK_HEAD_C, H, W, float(threshold),
                                _ptr(ws), _stream()), fn)
     return ge, gx
+
+
+FPN_C_MULTIPLE = 32     # the FPN upsample-add kernels take C a multiple of this
+
+
+def _fpn_nchw(t, name):
+    """-> (N, C, H, W) of an NCHW-contiguous CUDA float32 operand of the FPN upsample-add kernels, checked"""
+    if t.dim() != 4:
+        raise OdiseError(f"{name} must be [N, C, H, W], got {tuple(t.shape)}")
+    _req_shape(t, torch.float32, tuple(t.shape), name)
+    return tuple(t.shape)
+
+
+def _fpn_limits(N, C, h, w, H, W):
+    if min(N, C, h, w, H, W) <= 0:
+        raise OdiseError(f"FPN upsample-add: empty shape N={N}, C={C}, {h}x{w} -> {H}x{W}")
+    if C % FPN_C_MULTIPLE or N * (C // FPN_C_MULTIPLE) > 65535 or max(H, h) > 65535 or h * w * C >= 2 ** 31:
+        raise OdiseError(f"FPN upsample-add: N={N}, C={C}, {h}x{w} -> {H}x{W} not supported (C a multiple of "
+                         f"{FPN_C_MULTIPLE}, N * C / {FPN_C_MULTIPLE} <= 65535, H, h <= 65535, h*w*C < 2^31)")
+
+
+def _fpn_shapes(z, cur, size):
+    """Checks of fpn_upsample_add without data and without the library (the fake implementation in
+    odise_b200.pixel_decoder calls it too): z [N, h*w, C] float32 CUDA with channel-contiguous rows (strides
+    (>= h*w*C, C, 1); a token slice of the encoder's memory qualifies), cur [N, C, H, W] contiguous float32 CUDA.
+    -> (N, C, h, w, H, W, batch stride of z)"""
+    h, w = (int(s) for s in size)
+    N, C, H, W = _fpn_nchw(cur, "cur")
+    if not z.is_cuda or z.dtype != torch.float32:
+        raise OdiseError(f"z: expected a CUDA float32 tensor, got {z.dtype} on {z.device}")
+    if tuple(z.shape) != (N, h * w, C):
+        raise OdiseError(f"z: expected shape {(N, h * w, C)} (cur {(N, C, H, W)}, level {h}x{w}), got {tuple(z.shape)}")
+    _fpn_limits(N, C, h, w, H, W)
+    bs = z.stride(0) if N > 1 else h * w * C
+    if z.stride(2) != 1 or (h * w > 1 and z.stride(1) != C) or bs < h * w * C:
+        raise OdiseError(f"z: rows must be channel-contiguous with a batch stride >= h*w*C, got strides {z.stride()}")
+    return N, C, h, w, H, W, bs
+
+
+def fpn_upsample_add(z, cur, size):
+    """The pixel decoder's FPN step (odise_fpn_upsample_add_f32): cur + F.interpolate(level, cur's H x W, "bilinear",
+    align_corners=False) of the level z [N, h*w, C] (token-major, read in place; size = (h, w)) -> y [N, C, H, W],
+    bit-equal to torch's CUDA result.  OdiseError on CPU or non-float32 tensors, layouts and shapes the kernel does not
+    take."""
+    N, C, h, w, H, W, bs = _fpn_shapes(z, cur, size)
+    y = torch.empty_like(cur)
+    fn = "odise_fpn_upsample_add_f32"
+    _check(getattr(load(), fn)(_ptr(z), bs, _ptr(cur), _ptr(y), N, C, h, w, H, W, _stream()), fn)
+    return y
+
+
+def _fpn_backward_shapes(grad_y, size):
+    """Checks of fpn_upsample_add_backward (shared with its fake) -> (N, C, h, w, H, W)"""
+    h, w = (int(s) for s in size)
+    N, C, H, W = _fpn_nchw(grad_y, "grad_y")
+    _fpn_limits(N, C, h, w, H, W)
+    return N, C, h, w, H, W
+
+
+def fpn_upsample_add_backward(grad_y, size):
+    """Backward of fpn_upsample_add for the level (odise_fpn_upsample_add_backward_f32): grad_y [N, C, H, W]
+    contiguous float32 -> grad_z [N, h*w, C] contiguous, the adjoint of the bilinear resize, summed in a fixed order
+    without atomics (bit-reproducible).  The gradient of cur is grad_y itself."""
+    N, C, h, w, H, W = _fpn_backward_shapes(grad_y, size)
+    gz = torch.empty(N, h * w, C, dtype=torch.float32, device=grad_y.device)
+    fn = "odise_fpn_upsample_add_backward_f32"
+    _check(getattr(load(), fn)(_ptr(grad_y), _ptr(gz), h * w * C, N, C, h, w, H, W, _stream()), fn)
+    return gz
 
 
 class nvtx:

@@ -268,11 +268,19 @@ class MSDeformAttn(nn.Module):
         """query [N, Lq, C]; reference_points [N, Lq, L, 2] in [0, 1] (x, y) or [N, Lq, L, 4] boxes (x, y, w, h);
         input_flatten [N, S, C] with S = sum of H_l * W_l; input_spatial_shapes [L, 2] (H_l, W_l);
         input_level_start_index [L]; input_padding_mask [N, S], True at padding -> [N, Lq, C]."""
+        return self._attend(query, reference_points, input_flatten, input_spatial_shapes, input_level_start_index,
+                            input_padding_mask, check_shapes=True)
+
+    def _attend(self, query, reference_points, input_flatten, input_spatial_shapes, input_level_start_index,
+                input_padding_mask, check_shapes):
+        """forward(); check_shapes = False skips its host read of input_spatial_shapes (a synchronisation), for callers
+        that built the shapes from the same ints as input_flatten (odise_b200.pixel_decoder's encoder layers)"""
         if not (query.is_cuda and input_flatten.is_cuda and reference_points.is_cuda):
             raise lib.OdiseError("MSDeformAttn: expected CUDA tensors (odise_b200 kernels only run on the GPU)")
         N, Lq, _ = query.shape
         _, S, _ = input_flatten.shape
-        if not torch.compiler.is_compiling():  # reads the shapes on the host, which a traced graph cannot: skipped there
+        # reads the shapes on the host, which a traced graph cannot: skipped there
+        if check_shapes and not torch.compiler.is_compiling():
             assert (input_spatial_shapes[:, 0] * input_spatial_shapes[:, 1]).sum() == S
         M, L, P = self.n_heads, self.n_levels, self.n_points
         D = self.d_model // M
