@@ -32,8 +32,14 @@
 
 #include "launch_count.h"
 #include "odise_b200.h"
+#include "storage.cuh"
 
 namespace ob {
+
+// A target mask byte (bool or uint8, 0 / 1) as 0.f / 1.f, one more overload of storage.cuh's ld1.  It is declared in ob
+// itself: declared inside the anonymous namespace, it would hide the header's overloads from the kernels below.
+__device__ __forceinline__ float ld1(const uint8_t* p) { return __ldg(p) ? 1.f : 0.f; }
+
 namespace {
 
 constexpr int MC_TQ = 16;            // queries per cost CTA
@@ -41,14 +47,6 @@ constexpr int MC_TT = 16;            // targets per cost CTA
 constexpr int MC_CH = 128;           // points per cost chunk
 constexpr int MC_NT = 512;           // threads of the loss kernels
 constexpr int MC_SMEM_MAX = 227 * 1024;
-
-__device__ __forceinline__ float mc_ld(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float mc_ld(const __half* p) { return __half2float(__ldg(p)); }
-__device__ __forceinline__ float mc_ld(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
-__device__ __forceinline__ float mc_ld(const uint8_t* p) { return __ldg(p) ? 1.f : 0.f; }
-__device__ __forceinline__ void mc_st(float* p, double v) { *p = __double2float_rn(v); }
-__device__ __forceinline__ void mc_st(__half* p, double v) { *p = __double2half(v); }
-__device__ __forceinline__ void mc_st(__nv_bfloat16* p, double v) { *p = __double2bfloat16(v); }
 
 // bilinear corners of point (px, py) on an H x W map, as grid_sampler_2d_kernel computes them
 struct McCorners {
@@ -78,10 +76,10 @@ template <typename T>
 __device__ __forceinline__ float mc_sample(const T* map, int H, int W, float px, float py) {
   const McCorners c = mc_corners(px, py, H, W);
   float acc = 0.f;
-  if (mc_in(c.y0, c.x0, H, W)) acc = __fmaf_rn(c.w[0], mc_ld(map + (long long)c.y0 * W + c.x0), acc);
-  if (mc_in(c.y0, c.x0 + 1, H, W)) acc = __fmaf_rn(c.w[1], mc_ld(map + (long long)c.y0 * W + c.x0 + 1), acc);
-  if (mc_in(c.y0 + 1, c.x0, H, W)) acc = __fmaf_rn(c.w[2], mc_ld(map + (long long)(c.y0 + 1) * W + c.x0), acc);
-  if (mc_in(c.y0 + 1, c.x0 + 1, H, W)) acc = __fmaf_rn(c.w[3], mc_ld(map + (long long)(c.y0 + 1) * W + c.x0 + 1), acc);
+  if (mc_in(c.y0, c.x0, H, W)) acc = __fmaf_rn(c.w[0], ld1(map + (long long)c.y0 * W + c.x0), acc);
+  if (mc_in(c.y0, c.x0 + 1, H, W)) acc = __fmaf_rn(c.w[1], ld1(map + (long long)c.y0 * W + c.x0 + 1), acc);
+  if (mc_in(c.y0 + 1, c.x0, H, W)) acc = __fmaf_rn(c.w[2], ld1(map + (long long)(c.y0 + 1) * W + c.x0), acc);
+  if (mc_in(c.y0 + 1, c.x0 + 1, H, W)) acc = __fmaf_rn(c.w[3], ld1(map + (long long)(c.y0 + 1) * W + c.x0 + 1), acc);
   return acc;
 }
 
@@ -347,7 +345,7 @@ __global__ void __launch_bounds__(MC_NT) mc_loss_bwd_kernel(const T* __restrict_
   const long long n = __ldg(pair_of + bq);
   const int tid = threadIdx.x;
   if (n < 0) {
-    for (long long i = tid; i < HW; i += MC_NT) mc_st(out + i, 0.0);
+    for (long long i = tid; i < HW; i += MC_NT) st1d(out + i, 0.0);
     return;
   }
   const T* map = pred + bq * HW;
@@ -376,7 +374,7 @@ __global__ void __launch_bounds__(MC_NT) mc_loss_bwd_kernel(const T* __restrict_
   for (int i = 0; i < MC_NT / 32; ++i) gmax = fmaxf(gmax, red[i]);
   if (gmax == 0.f || !(gmax <= 3.0e38f)) {
     const double fill = gmax == 0.f ? 0.0 : (double)NAN;
-    for (long long i = tid; i < HW; i += MC_NT) mc_st(out + i, fill);
+    for (long long i = tid; i < HW; i += MC_NT) st1d(out + i, fill);
     return;
   }
   // every cell sums at most P contributions of |w g| <= gmax: below 2^e, so below 2^62 after scaling by 2^(62 - e)
@@ -401,7 +399,7 @@ __global__ void __launch_bounds__(MC_NT) mc_loss_bwd_kernel(const T* __restrict_
       }
     }
     __syncthreads();
-    for (int i = tid; i < cells; i += MC_NT) mc_st(out + (long long)r0 * W + i, (double)acc[i] * unscale);
+    for (int i = tid; i < cells; i += MC_NT) st1d(out + (long long)r0 * W + i, (double)acc[i] * unscale);
     __syncthreads();
   }
 }

@@ -29,6 +29,7 @@
 #include "launch_count.h"
 #include "mask_resize.cuh"
 #include "odise_b200.h"
+#include "storage.cuh"
 
 namespace ob {
 namespace {
@@ -42,10 +43,6 @@ constexpr int MH_KC = 32;                 // k per staged chunk of the backward 
 constexpr int MH_GS = MH_T + 4;           // row stride of the backward's staged tiles (float4 rows)
 constexpr int MH_TARGET_CTAS = 264;       // 2 per SM on 132 SMs: the split-K counts aim at this many CTAs
 constexpr size_t MH_FWD_SMEM = sizeof(float) * (MH_C * MH_T + MH_C * MH_XS + MH_T * MH_T);
-
-__device__ __forceinline__ void mh_st(float* p, float v) { *p = v; }
-__device__ __forceinline__ void mh_st(__half* p, float v) { *p = __float2half_rn(v); }
-__device__ __forceinline__ void mh_st(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
 template <typename T>
 __device__ __forceinline__ float mh_rnd(float v) { return mr_round(v, static_cast<T*>(nullptr)); }
@@ -132,7 +129,7 @@ mh_fwd_kernel(const T* __restrict__ E, const T* __restrict__ X, T* __restrict__ 
         float m = 0.f;
         if (q0 + q < Q && p0 + p < HW) {
           const float v = mh_rnd<T>(acc[j][i]);
-          mh_st(om + ((long long)b * Q + q0 + q) * HW + p0 + p, v);
+          st1(om + ((long long)b * Q + q0 + q) * HW + p0 + p, v);
           m = mh_hard<T>(v, thr);
         }
         Ms[q * MH_T + p] = m;
@@ -183,7 +180,7 @@ __global__ void mh_pool_finalize_kernel(const float* __restrict__ ws_pool, const
   // an empty mask pools nothing (the reference's operand m / denorm is 0 there); w = 0 also keeps fp16's
   // T(1 / 1e-8) = inf out of the products
   const float w = cnt > 0.f ? mh_rnd<T>(1.f / (cnt + 1e-8f)) : 0.f;
-  mh_st(pooled + i, sum * w);
+  st1(pooled + i, sum * w);
   if (i % MH_C == 0) weights[row] = w;
 }
 
@@ -285,7 +282,7 @@ __global__ void mh_grad_embed_reduce_kernel(const float* __restrict__ ws, T* __r
   if (i >= n) return;
   float sum = 0.f;
   for (int s = 0; s < splits; ++s) sum += ws[(long long)s * n + i];
-  mh_st(gE + i, sum);
+  st1(gE + i, sum);
 }
 
 // grid (pixel tiles, C / 64, B)
@@ -307,7 +304,7 @@ mh_grad_features_kernel(const T* __restrict__ E, const T* __restrict__ Gp, const
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const long long p = p0 + 4 * tx + i;
-      if (p < HW) mh_st(gX + ((long long)b * MH_C + c) * HW + p, acc[j][i]);
+      if (p < HW) st1(gX + ((long long)b * MH_C + c) * HW + p, acc[j][i]);
     }
   }
 }
@@ -413,7 +410,7 @@ mh_fwd_tc_kernel(const T* __restrict__ E, const T* __restrict__ X, T* __restrict
         bool m = false;
         if (q0 + q < Q && p0 + p < HW) {
           const float v = mh_rnd<T>(acc[j][e]);
-          mh_st(om + ((long long)b * Q + q0 + q) * HW + p0 + p, v);
+          st1(om + ((long long)b * Q + q0 + q) * HW + p0 + p, v);
           m = mh_hard<T>(v, thr) != 0.f;
         }
         Ms[q * MH_TC_LT + p] = m ? one : zero;
@@ -524,7 +521,7 @@ mh_grad_features_tc_kernel(const T* __restrict__ E, const T* __restrict__ Gp, co
     for (int e = 0; e < 4; ++e) {
       const int c = c0 + 16 * wm + g + 8 * (e >> 1);
       const long long p = p0 + 32 * wn + 8 * j + 2 * t4 + (e & 1);
-      if (p < HW) mh_st(gX + ((long long)b * MH_C + c) * HW + p, acc[j][e]);
+      if (p < HW) st1(gX + ((long long)b * MH_C + c) * HW + p, acc[j][e]);
     }
 }
 

@@ -26,6 +26,7 @@
 
 #include "launch_count.h"
 #include "odise_b200.h"
+#include "storage.cuh"
 
 namespace ob {
 namespace {
@@ -36,35 +37,6 @@ constexpr int XA_BK = 64;             // keys per shared-memory tile
 constexpr int XA_NT = 256;            // threads per CTA
 constexpr int XA_PS = XA_BK + 4;      // row stride of the P / dS tiles (float4-aligned)
 constexpr int XA_TARGET_CTAS = 528;   // 4 CTAs per SM on 132 SMs: the forward / dQ chunking aims at this many
-
-__device__ __forceinline__ float4 xa_ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-__device__ __forceinline__ float4 xa_ld4(const __half* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
-  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float4 xa_ld4(const __nv_bfloat16* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float xa_ld1(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float xa_ld1(const __half* p) { return __half2float(__ldg(p)); }
-__device__ __forceinline__ float xa_ld1(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
-__device__ __forceinline__ void xa_st1(float* p, float v) { *p = v; }
-__device__ __forceinline__ void xa_st1(__half* p, float v) { *p = __float2half_rn(v); }
-__device__ __forceinline__ void xa_st1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
-__device__ __forceinline__ void xa_st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-__device__ __forceinline__ void xa_st4(__half* p, float4 v) {
-  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-}
-__device__ __forceinline__ void xa_st4(__nv_bfloat16* p, float4 v) {
-  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-}
 
 __device__ __forceinline__ float4 xa_lds4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void xa_sts4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
@@ -77,7 +49,7 @@ __device__ __forceinline__ void xa_load_tile(float* dst, const T* src, long long
   for (int e = threadIdx.x; e < XA_BK * 8; e += XA_NT) {
     const int j = e >> 3, ch = e & 7;
     float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (k0 + j < S) x = xa_ld4(src + (long long)(k0 + j) * rs + ch * 4);
+    if (k0 + j < S) x = ld4(src + (long long)(k0 + j) * rs + ch * 4);
     xa_sts4(dst + j * XA_D + (SWZ ? (ch ^ (j >> 3)) : ch) * 4, x);
   }
 }
@@ -140,7 +112,7 @@ template <typename T>
 __device__ __forceinline__ void xa_row_regs(float* reg, const T* p, bool ok, float scale) {
 #pragma unroll
   for (int ch = 0; ch < 8; ++ch) {
-    float4 x = ok ? xa_ld4(p + ch * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 x = ok ? ld4(p + ch * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
     reg[4 * ch + 0] = x.x * scale;
     reg[4 * ch + 1] = x.y * scale;
     reg[4 * ch + 2] = x.z * scale;
@@ -259,7 +231,7 @@ __global__ void xattn_combine_kernel(const float* __restrict__ ws_acc, const flo
     ls = M + logf(L);
   }
   const long long E = sh.E();
-  xa_st1(out + (long long)qi * sh.B * E + (long long)b * E + h * XA_D + lane, o);
+  st1(out + (long long)qi * sh.B * E + (long long)b * E + h * XA_D + lane, o);
   if (lane == 0) lse[row] = ls;
 }
 
@@ -273,7 +245,7 @@ __global__ void xattn_delta_kernel(const T* __restrict__ out, const T* __restric
   if (row >= BHQ) return;
   const int bh = (int)(row / sh.Q), qi = (int)(row % sh.Q), b = bh / sh.H, h = bh % sh.H;
   const long long E = sh.E(), off = (long long)qi * sh.B * E + (long long)b * E + h * XA_D + lane;
-  float x = xa_ld1(dout + off) * xa_ld1(out + off);
+  float x = ld1(dout + off) * ld1(out + off);
 #pragma unroll
   for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
   if (lane == 0) delta[row] = x;
@@ -323,10 +295,10 @@ __global__ void __launch_bounds__(XA_NT, 2) xattn_bwd_dkdv_kernel(
       const int j = t >> 3, ch = t & 7;
       const bool ok = q0 + j < sh.Q;
       const long long off = (long long)(q0 + j) * rs + head + ch * 4;
-      float4 a = ok ? xa_ld4(q + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 a = ok ? ld4(q + off) : make_float4(0.f, 0.f, 0.f, 0.f);
       a.x *= scale; a.y *= scale; a.z *= scale; a.w *= scale;
       xa_sts4(Qs + j * XA_D + ch * 4, a);
-      xa_sts4(Ds + j * XA_D + ch * 4, ok ? xa_ld4(dout + off) : make_float4(0.f, 0.f, 0.f, 0.f));
+      xa_sts4(Ds + j * XA_D + ch * 4, ok ? ld4(dout + off) : make_float4(0.f, 0.f, 0.f, 0.f));
       if (t < XA_BQ) {
         const bool okr = q0 + t < sh.Q;
         lse_s[t] = okr ? lse[(long long)bh * sh.Q + q0 + t] : 0.f;
@@ -370,10 +342,10 @@ __global__ void __launch_bounds__(XA_NT, 2) xattn_bwd_dkdv_kernel(
   }
   if (k0 + kc < sh.S) {
     const long long off = (long long)(k0 + kc) * rs + head + dg;
-    xa_st4(dk + off, make_float4(dka[0], dka[1], dka[2], dka[3]));
-    xa_st4(dk + off + 4, make_float4(dka[4], dka[5], dka[6], dka[7]));
-    xa_st4(dv + off, make_float4(dva[0], dva[1], dva[2], dva[3]));
-    xa_st4(dv + off + 4, make_float4(dva[4], dva[5], dva[6], dva[7]));
+    st4(dk + off, make_float4(dka[0], dka[1], dka[2], dka[3]));
+    st4(dk + off + 4, make_float4(dka[4], dka[5], dka[6], dka[7]));
+    st4(dv + off, make_float4(dva[0], dva[1], dva[2], dva[3]));
+    st4(dv + off + 4, make_float4(dva[4], dva[5], dva[6], dva[7]));
   }
 }
 
@@ -444,7 +416,7 @@ __global__ void xattn_dq_reduce_kernel(const float* __restrict__ ws_dq, T* __res
   float a = 0.f;
   for (int c = 0; c < nchunk; ++c) a += ws_dq[(c * BHQ + row) * XA_D + c0];
   const long long E = sh.E();
-  xa_st1(dq + (long long)qi * sh.B * E + (long long)b * E + h * XA_D + c0, a * scale);
+  st1(dq + (long long)qi * sh.B * E + (long long)b * E + h * XA_D + c0, a * scale);
 }
 
 // key chunks of the forward and of the dQ pass: a function of the shape only

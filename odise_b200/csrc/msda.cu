@@ -13,6 +13,7 @@
 #include "ptx.cuh"
 #include "odise_b200.h"
 #include "launch_count.h"
+#include "storage.cuh"
 
 namespace ob {
 
@@ -22,52 +23,6 @@ struct MsdaLevels {
   const int64_t* shapes;
   const int64_t* start;
 };
-
-__device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-
-// Storage-type loads and stores of the D = 32 fused kernels (float, or 16-bit __half / __nv_bfloat16 under autocast).
-// A 16-bit load converts to float right after it (exact); a 16-bit store rounds the fp32 result once (round to nearest
-// even).  Everything in between is fp32.  Four 16-bit channels are one 64-bit load / store.
-__device__ __forceinline__ float4 ld4(const __half* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
-  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
-  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.x));
-  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-__device__ __forceinline__ float2 ld2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
-__device__ __forceinline__ float2 ld2(const __half* p) { return __half22float2(__ldg(reinterpret_cast<const __half2*>(p))); }
-__device__ __forceinline__ float2 ld2(const __nv_bfloat16* p) {
-  return __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(p)));
-}
-__device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float ld1(const __half* p) { return __half2float(__ldg(p)); }
-__device__ __forceinline__ float ld1(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
-
-__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-__device__ __forceinline__ void st4(__half* p, float4 v) {
-  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-}
-__device__ __forceinline__ void st4(__nv_bfloat16* p, float4 v) {
-  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-}
-__device__ __forceinline__ void st2(float* p, float2 v) { *reinterpret_cast<float2*>(p) = v; }
-__device__ __forceinline__ void st2(__half* p, float2 v) {
-  *reinterpret_cast<__half2*>(p) = __floats2half2_rn(v.x, v.y);
-}
-__device__ __forceinline__ void st2(__nv_bfloat16* p, float2 v) {
-  *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(v.x, v.y);
-}
-__device__ __forceinline__ void st1(float* p, float v) { *p = v; }
-__device__ __forceinline__ void st1(__half* p, float v) { *p = __float2half_rn(v); }
-__device__ __forceinline__ void st1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
 __device__ __forceinline__ void fma4(float4& acc, float w, const float4& v) {
   acc.x = fmaf(w, v.x, acc.x); acc.y = fmaf(w, v.y, acc.y); acc.z = fmaf(w, v.z, acc.z); acc.w = fmaf(w, v.w, acc.w);
@@ -734,11 +689,6 @@ msda_backward_warp_kernel(const T* __restrict__ value, const MsdaLevels lv, cons
 // their values, so atomicMax on the bits is deterministic; NaN (sign cleared) and +inf land at or above the bits of
 // +inf, which marks the slice non-finite.  Block b covers slice b / chunks; its warps take every (chunks * 8)-th query
 // row, the lanes stride over the row's `inner` elements.
-__device__ __forceinline__ double ld1d(const float* p) { return (double)__ldg(p); }
-__device__ __forceinline__ double ld1d(const double* p) { return __ldg(p); }
-__device__ __forceinline__ double ld1d(const __half* p) { return (double)__half2float(__ldg(p)); }
-__device__ __forceinline__ double ld1d(const __nv_bfloat16* p) { return (double)__bfloat162float(__ldg(p)); }
-
 template <typename T>
 __global__ void __launch_bounds__(256)
 msda_absmax_kernel(const T* __restrict__ x, unsigned long long* __restrict__ out, int M, int Lq, int inner,
@@ -755,11 +705,6 @@ msda_absmax_kernel(const T* __restrict__ x, unsigned long long* __restrict__ out
   for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   if (lane == 0 && mx) atomicMax(out + nm, mx);
 }
-
-__device__ __forceinline__ void st1d(float* p, double v) { *p = (float)v; }
-__device__ __forceinline__ void st1d(double* p, double v) { *p = v; }
-__device__ __forceinline__ void st1d(__half* p, double v) { *p = __double2half(v); }
-__device__ __forceinline__ void st1d(__nv_bfloat16* p, double v) { *p = __double2bfloat16(v); }
 
 // Finalize: grad_value[n, i, m, c] = sum * 2^-s of its (n, m) slice in Tout; NaN in a non-finite slice.  The sum goes to
 // double exactly while |sum| <= 2^53 and is then rounded once to Tout; a larger sum is rounded to double first (two
@@ -786,50 +731,57 @@ msda_fixed_finalize_kernel(const MsdaFixedAcc acc, Tout* __restrict__ grad_value
 
 using namespace ob;
 
-extern "C" int odise_msda_forward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                      const float* loc, const float* attn, float* out, int N, int S, int M, int D,
-                                      int L, int Lq, int P, void* stream_v) {
+// float: the D = 32 kernel where d32_ok, else the vec4 kernel where vec_ok(D), else the scalar kernel.  double: the
+// scalar kernel for every D.
+template <typename T>
+static int msda_forward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start, const T* loc,
+                        const T* attn, T* out, int N, int S, int M, int D, int L, int Lq, int P, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value || !spatial_shapes || !level_start || !loc || !attn || !out) return ODISE_ERR_ARG;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
   MsdaLevels lv{spatial_shapes, level_start};
-  if (d32_ok(S, M, D, L, P)) {
-    launch_d32<0>(value, lv, loc, attn, nullptr, out, nullptr, nullptr, N, S, M, L, Lq, P, stream);
-  } else if (vec_ok(D)) {
-    const int lph = D / 4;
-    const long long threads = (long long)N * Lq * M * lph;
-    const int blocks = (int)((threads + 255) / 256);
-    msda_vec4_kernel<0><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, nullptr, out, nullptr, nullptr, N, S, M, D,
-                                                    L, Lq, P, lph);
-  } else {
+  bool launched = false;
+  if constexpr (std::is_same<T, float>::value) {
+    if (d32_ok(S, M, D, L, P)) {
+      launch_d32<0>(value, lv, loc, attn, nullptr, out, nullptr, nullptr, N, S, M, L, Lq, P, stream);
+      launched = true;
+    } else if (vec_ok(D)) {
+      const int lph = D / 4;
+      const long long threads = (long long)N * Lq * M * lph;
+      const int blocks = (int)((threads + 255) / 256);
+      msda_vec4_kernel<0><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, nullptr, out, nullptr, nullptr, N, S, M, D,
+                                                      L, Lq, P, lph);
+      launched = true;
+    }
+  }
+  if (!launched) {
     const long long total = (long long)N * Lq * M * D;
     int blocks = (int)((total + 255) / 256);
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-    msda_scalar_kernel<float><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
+    msda_scalar_kernel<T><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
   }
   count_launch(1);
   return (int)cudaGetLastError();
 }
 
-extern "C" int odise_msda_forward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                      const double* loc, const double* attn, double* out, int N, int S, int M, int D,
-                                      int L, int Lq, int P, void* stream_v) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-  if (!value || !spatial_shapes || !level_start || !loc || !attn || !out) return ODISE_ERR_ARG;
-  if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
-  MsdaLevels lv{spatial_shapes, level_start};
-  const long long total = (long long)N * Lq * M * D;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-  msda_scalar_kernel<double><<<blocks, 256, 0, stream>>>(value, lv, loc, attn, out, N, S, M, D, L, Lq, P);
-  count_launch(1);
-  return (int)cudaGetLastError();
-}
+#define MSDA_FORWARD(sfx, T)                                                                                           \
+  extern "C" int odise_msda_forward_##sfx(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,   \
+                                          const T* loc, const T* attn, T* out, int N, int S, int M, int D, int L,      \
+                                          int Lq, int P, void* stream) {                                               \
+    return msda_forward<T>(value, spatial_shapes, level_start, loc, attn, out, N, S, M, D, L, Lq, P, stream);          \
+  }
+MSDA_FORWARD(f32, float)
+MSDA_FORWARD(f64, double)
 
 // Workspace of the deterministic backward entry points (odise_msda_det_workspace_bytes): the int64 sums [N, S, M, D],
 // then per (n, m) the max-|grad_out| and max-|attn| bits of MsdaFixedAcc.
 static long long det_ws_bytes(int N, int S, int M, int D) {
   return (long long)sizeof(unsigned long long) * ((long long)N * S * M * D + 2LL * N * M);
+}
+
+extern "C" long long odise_msda_det_workspace_bytes(int N, int S, int M, int D) {
+  if (N <= 0 || S <= 0 || M <= 0 || D <= 0) return 0;
+  return det_ws_bytes(N, S, M, D);
 }
 
 static MsdaFixedAcc det_acc(void* ws, int N, int S, int M, int D, int Lq, int P) {
@@ -923,44 +875,24 @@ static int msda_backward(const T* value, const int64_t* spatial_shapes, const in
   return (int)cudaGetLastError();
 }
 
-extern "C" int odise_msda_backward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                       const float* loc, const float* attn, const float* grad_out, float* grad_value,
-                                       float* grad_loc, float* grad_attn, int N, int S, int M, int D, int L, int Lq,
-                                       int P, void* stream) {
-  return msda_backward<float>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,
-                              N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" int odise_msda_backward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                       const double* loc, const double* attn, const double* grad_out,
-                                       double* grad_value, double* grad_loc, double* grad_attn, int N, int S, int M,
-                                       int D, int L, int Lq, int P, void* stream) {
-  return msda_backward<double>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc,
-                               grad_attn, N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" long long odise_msda_det_workspace_bytes(int N, int S, int M, int D) {
-  if (N <= 0 || S <= 0 || M <= 0 || D <= 0) return 0;
-  return det_ws_bytes(N, S, M, D);
-}
-
-extern "C" int odise_msda_backward_det_f32(const float* value, const int64_t* spatial_shapes,
-                                           const int64_t* level_start, const float* loc, const float* attn,
-                                           const float* grad_out, float* grad_value, float* grad_loc, float* grad_attn,
-                                           int N, int S, int M, int D, int L, int Lq, int P, void* workspace,
-                                           void* stream) {
-  return msda_backward<float>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,
-                              N, S, M, D, L, Lq, P, true, workspace, stream);
-}
-
-extern "C" int odise_msda_backward_det_f64(const double* value, const int64_t* spatial_shapes,
-                                           const int64_t* level_start, const double* loc, const double* attn,
-                                           const double* grad_out, double* grad_value, double* grad_loc,
-                                           double* grad_attn, int N, int S, int M, int D, int L, int Lq, int P,
-                                           void* workspace, void* stream) {
-  return msda_backward<double>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc,
-                               grad_attn, N, S, M, D, L, Lq, P, true, workspace, stream);
-}
+#define MSDA_BACKWARD(sfx, T)                                                                                          \
+  extern "C" int odise_msda_backward_##sfx(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,  \
+                                           const T* loc, const T* attn, const T* grad_out, T* grad_value,              \
+                                           T* grad_loc, T* grad_attn, int N, int S, int M, int D, int L, int Lq,       \
+                                           int P, void* stream) {                                                      \
+    return msda_backward<T>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,  \
+                            N, S, M, D, L, Lq, P, false, nullptr, stream);                                             \
+  }                                                                                                                    \
+  extern "C" int odise_msda_backward_det_##sfx(const T* value, const int64_t* spatial_shapes,                          \
+                                               const int64_t* level_start, const T* loc, const T* attn,                \
+                                               const T* grad_out, T* grad_value, T* grad_loc, T* grad_attn, int N,     \
+                                               int S, int M, int D, int L, int Lq, int P, void* workspace,             \
+                                               void* stream) {                                                         \
+    return msda_backward<T>(value, spatial_shapes, level_start, loc, attn, grad_out, grad_value, grad_loc, grad_attn,  \
+                            N, S, M, D, L, Lq, P, true, workspace, stream);                                            \
+  }
+MSDA_BACKWARD(f32, float)
+MSDA_BACKWARD(f64, double)
 
 extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
                                     const float* ref, const float* offs, const float* logits, float* out,
@@ -988,12 +920,13 @@ extern "C" int odise_msda_fused_f32(const float* value, const int64_t* spatial_s
 // a box reference point [N, Lq, L, 4] is one 16-byte load
 static bool ref_ok(const float* ref, int RW) { return RW == 2 || reinterpret_cast<uintptr_t>(ref) % 16 == 0; }
 
-// The fused forward on the D = 32 kernel only, no planes: a 16-bit storage type T (odise_msda_fused_f16 / _bf16), and
-// with RW = 4 the box forms for every T (odise_msda_fused_box_f32 / _f16 / _bf16).
-template <typename T, int RW = 2>
-static int msda_fused_16(const void* value_v, const int64_t* spatial_shapes, const int64_t* level_start,
-                         const float* ref, const void* offs_v, const void* logits_v, void* out_v, int N, int S, int M,
-                         int D, int L, int Lq, int P, void* stream_v) {
+// The fused forward on the D = 32 kernel alone, without planes: 16-bit storage T with RW = 2 (odise_msda_fused_f16 /
+// _bf16), and box reference points [N, Lq, L, 4] (cx, cy, w, h) with RW = 4 in every storage type
+// (odise_msda_fused_box_f32 / _f16 / _bf16; include/odise_b200.h states the formulas).
+template <typename T, int RW>
+static int msda_fused_d32(const void* value_v, const int64_t* spatial_shapes, const int64_t* level_start,
+                          const float* ref, const void* offs_v, const void* logits_v, void* out_v, int N, int S, int M,
+                          int D, int L, int Lq, int P, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
   if (!value_v || !spatial_shapes || !level_start || !ref || !offs_v || !logits_v || !out_v) return ODISE_ERR_ARG;
   if (N <= 0 || S <= 0 || M <= 0 || D <= 0 || L <= 0 || L > 8 || Lq <= 0 || P <= 0) return ODISE_ERR_ARG;
@@ -1008,28 +941,33 @@ static int msda_fused_16(const void* value_v, const int64_t* spatial_shapes, con
   return (int)cudaGetLastError();
 }
 
-extern "C" int odise_msda_fused_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                    const float* ref, const void* offs, const void* logits, void* out, int N, int S,
-                                    int M, int D, int L, int Lq, int P, void* stream) {
-  return msda_fused_16<__half>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P, stream);
-}
-
-extern "C" int odise_msda_fused_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                     const float* ref, const void* offs, const void* logits, void* out, int N, int S,
-                                     int M, int D, int L, int Lq, int P, void* stream) {
-  return msda_fused_16<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
-                                      stream);
-}
+// Arg: what the entry point's storage pointers point to (float, or void for 16-bit storage).
+#define MSDA_FUSED_D32(kind, sfx, Arg, T, RW)                                                                          \
+  extern "C" int odise_msda_##kind##_##sfx(const Arg* value, const int64_t* spatial_shapes,                            \
+                                           const int64_t* level_start, const float* ref, const Arg* offs,              \
+                                           const Arg* logits, Arg* out, int N, int S, int M, int D, int L, int Lq,     \
+                                           int P, void* stream) {                                                      \
+    return msda_fused_d32<T, RW>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,     \
+                                 stream);                                                                              \
+  }
+MSDA_FUSED_D32(fused, f16, void, __half, 2)
+MSDA_FUSED_D32(fused, bf16, void, __nv_bfloat16, 2)
+MSDA_FUSED_D32(fused_box, f32, float, float, 4)
+MSDA_FUSED_D32(fused_box, f16, void, __half, 4)
+MSDA_FUSED_D32(fused_box, bf16, void, __nv_bfloat16, 4)
 
 // The fused backward for storage type T.  Default (det = false): grad_value is an fp32 buffer for every T, accumulated
-// with fp32 atomics.  det = true: grad_value is in T, written by the fixed-point finalize pass through `ws`.  RW = 4: box
-// reference points (odise_msda_fused_box_backward_*).
-template <typename T, int RW = 2>
-static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                               const float* ref, const T* offs, const T* logits, const T* grad_out, void* grad_value,
-                               T* grad_offs, T* grad_logits, int N, int S, int M, int D, int L, int Lq, int P,
-                               bool det, void* ws, void* stream_v) {
+// with fp32 atomics.  det = true: grad_value is in T, written by the fixed-point finalize pass through `ws`.  RW = 4:
+// box reference points.
+template <typename T, int RW>
+static int msda_fused_backward(const void* value_v, const int64_t* spatial_shapes, const int64_t* level_start,
+                               const float* ref, const void* offs_v, const void* logits_v, const void* grad_out_v,
+                               void* grad_value, void* grad_offs_v, void* grad_logits_v, int N, int S, int M, int D,
+                               int L, int Lq, int P, bool det, void* ws, void* stream_v) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+  const T *value = static_cast<const T*>(value_v), *offs = static_cast<const T*>(offs_v);
+  const T *logits = static_cast<const T*>(logits_v), *grad_out = static_cast<const T*>(grad_out_v);
+  T *grad_offs = static_cast<T*>(grad_offs_v), *grad_logits = static_cast<T*>(grad_logits_v);
   if (!value || !spatial_shapes || !level_start || !ref || !offs || !logits || !grad_out || !grad_value || !grad_offs ||
       !grad_logits)
     return ODISE_ERR_ARG;
@@ -1069,167 +1007,26 @@ static int msda_fused_backward(const T* value, const int64_t* spatial_shapes, co
   return (int)cudaGetLastError();
 }
 
-extern "C" int odise_msda_fused_backward_f32(const float* value, const int64_t* spatial_shapes,
-                                             const int64_t* level_start, const float* ref, const float* offs,
-                                             const float* logits, const float* grad_out, float* grad_value,
-                                             float* grad_offs, float* grad_logits, int N, int S, int M, int D, int L,
-                                             int Lq, int P, void* stream) {
-  return msda_fused_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" int odise_msda_fused_backward_f16(const void* value, const int64_t* spatial_shapes,
-                                             const int64_t* level_start, const float* ref, const void* offs,
-                                             const void* logits, const void* grad_out, float* grad_value,
-                                             void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
-                                             int Lq, int P, void* stream) {
-  using T = __half;
-  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
-                                static_cast<const T*>(offs), static_cast<const T*>(logits),
-                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" int odise_msda_fused_backward_bf16(const void* value, const int64_t* spatial_shapes,
-                                              const int64_t* level_start, const float* ref, const void* offs,
-                                              const void* logits, const void* grad_out, float* grad_value,
-                                              void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
-                                              int Lq, int P, void* stream) {
-  using T = __nv_bfloat16;
-  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
-                                static_cast<const T*>(offs), static_cast<const T*>(logits),
-                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-// Deterministic twins of the fused backward: arguments of the default entry points plus the workspace; grad_value in
+// The default entry point takes grad_value in fp32; its deterministic twin adds the workspace and takes grad_value in
 // the storage type.
-extern "C" int odise_msda_fused_backward_det_f32(const float* value, const int64_t* spatial_shapes,
-                                                 const int64_t* level_start, const float* ref, const float* offs,
-                                                 const float* logits, const float* grad_out, float* grad_value,
-                                                 float* grad_offs, float* grad_logits, int N, int S, int M, int D,
-                                                 int L, int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                    grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
-}
-
-template <typename T>
-static int msda_fused_backward_det_16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                      const float* ref, const void* offs, const void* logits, const void* grad_out,
-                                      void* grad_value, void* grad_offs, void* grad_logits, int N, int S, int M, int D,
-                                      int L, int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_backward<T>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
-                                static_cast<const T*>(offs), static_cast<const T*>(logits),
-                                static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, true, workspace, stream);
-}
-
-extern "C" int odise_msda_fused_backward_det_f16(const void* value, const int64_t* spatial_shapes,
-                                                 const int64_t* level_start, const float* ref, const void* offs,
-                                                 const void* logits, const void* grad_out, void* grad_value,
-                                                 void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
-                                                 int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_backward_det_16<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
-                                            grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, workspace,
-                                            stream);
-}
-
-extern "C" int odise_msda_fused_backward_det_bf16(const void* value, const int64_t* spatial_shapes,
-                                                  const int64_t* level_start, const float* ref, const void* offs,
-                                                  const void* logits, const void* grad_out, void* grad_value,
-                                                  void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
-                                                  int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_backward_det_16<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
-                                                   grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, workspace,
-                                                   stream);
-}
-
-// Box reference points [N, Lq, L, 4] (cx, cy, w, h): the fused entry points above with RW = 4, on the D = 32 kernels in
-// every storage type (include/odise_b200.h states the formulas).
-extern "C" int odise_msda_fused_box_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                        const float* ref, const float* offs, const float* logits, float* out, int N,
-                                        int S, int M, int D, int L, int Lq, int P, void* stream) {
-  return msda_fused_16<float, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
-                                 stream);
-}
-
-extern "C" int odise_msda_fused_box_f16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                        const float* ref, const void* offs, const void* logits, void* out, int N, int S,
-                                        int M, int D, int L, int Lq, int P, void* stream) {
-  return msda_fused_16<__half, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq, P,
-                                  stream);
-}
-
-extern "C" int odise_msda_fused_box_bf16(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                         const float* ref, const void* offs, const void* logits, void* out, int N,
-                                         int S, int M, int D, int L, int Lq, int P, void* stream) {
-  return msda_fused_16<__nv_bfloat16, 4>(value, spatial_shapes, level_start, ref, offs, logits, out, N, S, M, D, L, Lq,
-                                         P, stream);
-}
-
-template <typename T>
-static int msda_fused_box_backward(const void* value, const int64_t* spatial_shapes, const int64_t* level_start,
-                                   const float* ref, const void* offs, const void* logits, const void* grad_out,
-                                   void* grad_value, void* grad_offs, void* grad_logits, int N, int S, int M, int D,
-                                   int L, int Lq, int P, bool det, void* workspace, void* stream) {
-  return msda_fused_backward<T, 4>(static_cast<const T*>(value), spatial_shapes, level_start, ref,
-                                   static_cast<const T*>(offs), static_cast<const T*>(logits),
-                                   static_cast<const T*>(grad_out), grad_value, static_cast<T*>(grad_offs),
-                                   static_cast<T*>(grad_logits), N, S, M, D, L, Lq, P, det, workspace, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_f32(const float* value, const int64_t* spatial_shapes,
-                                                 const int64_t* level_start, const float* ref, const float* offs,
-                                                 const float* logits, const float* grad_out, float* grad_value,
-                                                 float* grad_offs, float* grad_logits, int N, int S, int M, int D,
-                                                 int L, int Lq, int P, void* stream) {
-  return msda_fused_box_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                        grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_f16(const void* value, const int64_t* spatial_shapes,
-                                                 const int64_t* level_start, const float* ref, const void* offs,
-                                                 const void* logits, const void* grad_out, float* grad_value,
-                                                 void* grad_offs, void* grad_logits, int N, int S, int M, int D, int L,
-                                                 int Lq, int P, void* stream) {
-  return msda_fused_box_backward<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                         grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_bf16(const void* value, const int64_t* spatial_shapes,
-                                                  const int64_t* level_start, const float* ref, const void* offs,
-                                                  const void* logits, const void* grad_out, float* grad_value,
-                                                  void* grad_offs, void* grad_logits, int N, int S, int M, int D,
-                                                  int L, int Lq, int P, void* stream) {
-  return msda_fused_box_backward<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
-                                                grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, false,
-                                                nullptr, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_det_f32(const float* value, const int64_t* spatial_shapes,
-                                                     const int64_t* level_start, const float* ref, const float* offs,
-                                                     const float* logits, const float* grad_out, float* grad_value,
-                                                     float* grad_offs, float* grad_logits, int N, int S, int M, int D,
-                                                     int L, int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_box_backward<float>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                        grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_det_f16(const void* value, const int64_t* spatial_shapes,
-                                                     const int64_t* level_start, const float* ref, const void* offs,
-                                                     const void* logits, const void* grad_out, void* grad_value,
-                                                     void* grad_offs, void* grad_logits, int N, int S, int M, int D,
-                                                     int L, int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_box_backward<__half>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,
-                                         grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);
-}
-
-extern "C" int odise_msda_fused_box_backward_det_bf16(const void* value, const int64_t* spatial_shapes,
-                                                      const int64_t* level_start, const float* ref, const void* offs,
-                                                      const void* logits, const void* grad_out, void* grad_value,
-                                                      void* grad_offs, void* grad_logits, int N, int S, int M, int D,
-                                                      int L, int Lq, int P, void* workspace, void* stream) {
-  return msda_fused_box_backward<__nv_bfloat16>(value, spatial_shapes, level_start, ref, offs, logits, grad_out,
-                                                grad_value, grad_offs, grad_logits, N, S, M, D, L, Lq, P, true,
-                                                workspace, stream);
-}
+#define MSDA_FUSED_BACKWARD(kind, sfx, Arg, T, RW)                                                                     \
+  extern "C" int odise_msda_##kind##_backward_##sfx(                                                                   \
+      const Arg* value, const int64_t* spatial_shapes, const int64_t* level_start, const float* ref, const Arg* offs,  \
+      const Arg* logits, const Arg* grad_out, float* grad_value, Arg* grad_offs, Arg* grad_logits, int N, int S,       \
+      int M, int D, int L, int Lq, int P, void* stream) {                                                              \
+    return msda_fused_backward<T, RW>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,     \
+                                      grad_offs, grad_logits, N, S, M, D, L, Lq, P, false, nullptr, stream);           \
+  }                                                                                                                    \
+  extern "C" int odise_msda_##kind##_backward_det_##sfx(                                                               \
+      const Arg* value, const int64_t* spatial_shapes, const int64_t* level_start, const float* ref, const Arg* offs,  \
+      const Arg* logits, const Arg* grad_out, Arg* grad_value, Arg* grad_offs, Arg* grad_logits, int N, int S,         \
+      int M, int D, int L, int Lq, int P, void* workspace, void* stream) {                                             \
+    return msda_fused_backward<T, RW>(value, spatial_shapes, level_start, ref, offs, logits, grad_out, grad_value,     \
+                                      grad_offs, grad_logits, N, S, M, D, L, Lq, P, true, workspace, stream);          \
+  }
+MSDA_FUSED_BACKWARD(fused, f32, float, float, 2)
+MSDA_FUSED_BACKWARD(fused, f16, void, __half, 2)
+MSDA_FUSED_BACKWARD(fused, bf16, void, __nv_bfloat16, 2)
+MSDA_FUSED_BACKWARD(fused_box, f32, float, float, 4)
+MSDA_FUSED_BACKWARD(fused_box, f16, void, __half, 4)
+MSDA_FUSED_BACKWARD(fused_box, bf16, void, __nv_bfloat16, 4)
