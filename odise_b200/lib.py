@@ -5,7 +5,8 @@ the C ABI.  There is NO fallback: if the library is missing or a call fails, an 
 """
 import ctypes
 import os
-from ctypes import c_int, c_float, c_longlong, c_void_p, POINTER
+import re
+from ctypes import c_double, c_float, c_int, c_longlong, c_void_p, POINTER
 
 import torch
 
@@ -19,172 +20,58 @@ class OdiseError(RuntimeError):
     pass
 
 
-class GemmDesc(ctypes.Structure):
-    _fields_ = [
-        ("M", c_int), ("N", c_int), ("K", c_int), ("batch", c_int),
-        ("nmma", c_int), ("conv3x3", c_int),
-        ("conv_C", c_int), ("conv_H", c_int), ("conv_W", c_int),
-        ("a_hi", c_void_p), ("a_lo", c_void_p), ("lda", c_longlong), ("a_batch_stride", c_longlong),
-        ("b_hi", c_void_p), ("b_lo", c_void_p), ("ldb", c_longlong), ("b_batch_stride", c_longlong),
-        ("alpha", c_float),
-        ("bias", c_void_p),
-        ("rowbias", c_void_p), ("rows_per_group", c_int), ("rowbias_ld", c_longlong),
-        ("act", c_int),
-        ("residual", c_void_p), ("ld_residual", c_longlong), ("residual_batch_stride", c_longlong),
-        ("out_f32", c_void_p), ("ld_out", c_longlong), ("out_batch_stride", c_longlong),
-        ("out_hi", c_void_p), ("out_lo", c_void_p), ("ld_out_bf16", c_longlong), ("out_bf16_batch_stride", c_longlong),
-        ("split_k", c_int), ("workspace", c_void_p), ("workspace_bytes", c_longlong),
-        ("force_bn", c_int),
-        ("bias_m", c_void_p),
-        ("conv_mode", c_int),
-        ("geglu", c_int),
-        ("gn_partial", c_void_p), ("gn_seg_stride", c_longlong), ("gn_plane_stride", c_longlong),
-        ("out_planes_fp16", c_int),
-    ]
+_HEADER = os.path.normpath(os.path.join(_HERE, os.pardir, "include", "odise_b200.h"))
+# the C scalar types the header may use; any other non-pointer type is an error, never a guess
+_SCALARS = {"int": c_int, "long long": c_longlong, "int64_t": c_longlong, "float": c_float, "double": c_double}
 
+
+def _decls(decl, structs):
+    """[(name, ctypes type)] of one C declaration: a parameter "const float* x" or a field statement "int M, N, K".
+    const is dropped; a pointer to a struct in `structs` is POINTER(that Structure), any other pointer c_void_p."""
+    err = f"{_HEADER}: no ctypes type for `{' '.join(decl.split())}`"
+    first, *more = [d.strip() for d in decl.split(",")]
+    m = re.fullmatch(r"([\w\s]+?)\s*(\*?\s*\w+)", first)
+    if m is None:
+        raise OdiseError(err)
+    base = " ".join(w for w in m.group(1).split() if w != "const")
+    out = []
+    for d in [m.group(2)] + more:
+        dm = re.fullmatch(r"(\*?)\s*(\w+)", d)
+        if dm is None or not (dm.group(1) or base in _SCALARS):
+            raise OdiseError(err)
+        if dm.group(1):
+            out.append((dm.group(2), POINTER(structs[base]) if base in structs else c_void_p))
+        else:
+            out.append((dm.group(2), _SCALARS[base]))
+    return out
+
+
+def _parse_header(text):
+    """-> (structs, protos) of the C ABI header's text: each `typedef struct {...} name;` as a ctypes.Structure class
+    called `name`, and name -> (restype, argtypes) of each odise_* prototype."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^\s*#.*$", "", text, flags=re.M)
+    structs = {}
+    for body, name in re.findall(r"typedef\s+struct\s*\w*\s*\{([^}]*)\}\s*(\w+)\s*;", text):
+        fields = [f for stmt in body.split(";") if stmt.strip() for f in _decls(stmt, structs)]
+        structs[name] = type(name, (ctypes.Structure,), {"_fields_": fields})
+    protos = {}
+    for ret, name, args in re.findall(r"([\w\s*]+?)\b(odise_\w+)\s*\(([^()]*)\)\s*;", text):
+        argtypes = [] if args.strip() == "void" else [_decls(a, structs)[0][1] for a in args.split(",")]
+        protos[name] = (_decls(f"{ret} {name}", structs)[0][1], argtypes)
+    return structs, protos
+
+
+# every signature and struct layout comes from include/odise_b200.h, the one statement of the ABI the .cu files compile
+# against: a new entry point is declared there only
+if not os.path.exists(_HEADER):
+    raise OdiseError(f"{_HEADER} not found: odise_b200/lib.py binds the library from its declarations")
+with open(_HEADER) as _f:
+    _STRUCTS, _PROTOS = _parse_header(_f.read())
+GemmDesc = _STRUCTS["odise_gemm_desc"]
+PostprocessGeom = _STRUCTS["odise_postprocess_geom"]     # sem_seg_postprocess's padded size and un-padded image size
 
 _lib = None
-
-# name -> argtypes (all return int); kept in one place so tests can check every header symbol is bound
-_SIGS = {
-    "odise_msda_forward_f32": [c_void_p] * 6 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
-    "odise_msda_forward_f64": [c_void_p] * 6 + [c_int] * 7 + [c_void_p],
-    "odise_msda_backward_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
-    "odise_msda_backward_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_backward_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_f16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_bf16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_backward_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_backward_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_det_workspace_bytes": [c_int] * 4,           # returns long long (set in load())
-    "odise_msda_backward_det_f32": [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_backward_det_f64": [c_void_p] * 9 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_box_f32": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_f16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_bf16": [c_void_p] * 7 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_backward_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_backward_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_backward_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p],
-    "odise_msda_fused_box_backward_det_f32": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_box_backward_det_f16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_msda_fused_box_backward_det_bf16": [c_void_p] * 10 + [c_int] * 7 + [c_void_p, c_void_p],
-    "odise_masked_xattn_workspace_bytes": [c_int] * 4,       # returns long long (set in load())
-    "odise_masked_xattn_forward_f32": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_masked_xattn_forward_f16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_masked_xattn_forward_bf16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_masked_xattn_backward_f32": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_masked_xattn_backward_f16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_masked_xattn_backward_bf16": [c_void_p] * 4 + [c_longlong] + [c_void_p] * 6 + [c_int] * 5 + [c_void_p] * 2,
-    "odise_mask_loss_workspace_bytes": [c_int] * 2,          # returns long long (set in load())
-    "odise_mask_cost_f32": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
-    "odise_mask_cost_f16": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
-    "odise_mask_cost_bf16": [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p],
-    "odise_mask_point_sample_f32": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
-    "odise_mask_point_sample_f16": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
-    "odise_mask_point_sample_bf16": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
-    "odise_mask_point_sample_u8": [c_void_p] * 3 + [c_int] * 4 + [c_void_p],
-    "odise_mask_loss_forward_f32": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
-    "odise_mask_loss_forward_f16": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
-    "odise_mask_loss_forward_bf16": [c_void_p] * 7 + [c_int] * 10 + [c_float, c_void_p],
-    "odise_mask_loss_backward_f32": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
-    "odise_mask_loss_backward_f16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
-    "odise_mask_loss_backward_bf16": [c_void_p] * 7 + [c_int] * 8 + [c_float, c_void_p],
-    "odise_mask_head_workspace_bytes": [c_int] * 5,          # returns long long (set in load())
-    "odise_mask_head_forward_f32": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_mask_head_forward_f16": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_mask_head_forward_bf16": [c_void_p] * 5 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_mask_head_attn_mask_f32": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
-    "odise_mask_head_attn_mask_f16": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
-    "odise_mask_head_attn_mask_bf16": [c_void_p] * 2 + [c_int] * 7 + [c_void_p],
-    "odise_mask_head_backward_f32": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_mask_head_backward_f16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_mask_head_backward_bf16": [c_void_p] * 8 + [c_int] * 5 + [c_float, c_void_p, c_void_p],
-    "odise_fpn_upsample_add_f32": [c_void_p, c_longlong, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p],
-    "odise_fpn_upsample_add_backward_f32": [c_void_p, c_void_p, c_longlong] + [c_int] * 6 + [c_void_p],
-    "odise_gemm_bf16": [POINTER(GemmDesc), c_void_p],
-    "odise_gemm_tile_policy": [c_int] * 6 + [c_void_p, c_void_p],
-    "odise_profile_begin": [],
-    "odise_profile_end": [c_void_p, c_void_p, c_void_p],
-    "odise_split_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_void_p],
-    "odise_split_f16_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_void_p],
-    "odise_groupnorm_stats_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
-                                  c_void_p],
-    "odise_groupnorm_apply_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
-                                  c_longlong, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_groupnorm_finalize_seg_f32": [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                         c_float, c_void_p],
-    "odise_groupnorm_stats_bs_f32": [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                     c_float, c_void_p],
-    "odise_groupnorm_stats_ws_f32": [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                     c_int, c_int, c_float, c_void_p],
-    "odise_groupnorm_apply_bs_f32": [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                                     c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong,
-                                     c_int, c_int, c_int, c_int, c_void_p],
-    "odise_resize_nhwc_bs_f32": [c_void_p, c_longlong, c_longlong, c_void_p, c_longlong, c_longlong, c_int, c_int,
-                                 c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_groupnorm_apply_res_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_longlong, c_int, c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_longlong,
-                                      c_int, c_int, c_int, c_int, c_void_p],
-    "odise_bcast_fma_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
-    "odise_rowscale_f32": [c_void_p, c_longlong, c_void_p, c_longlong, c_int, c_void_p],
-    "odise_layernorm_f32": [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_float, c_void_p,
-                            c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int,
-                            c_void_p],
-    "odise_geglu_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_void_p],
-    "odise_add_split_f32": [c_void_p, c_longlong, c_void_p, c_longlong, c_longlong, c_void_p, c_longlong, c_void_p,
-                            c_void_p, c_longlong, c_longlong, c_int, c_void_p],
-    "odise_upsample2x_split_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int,
-                                   c_void_p],
-    "odise_im2col3x3_split_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                                  c_int, c_int, c_void_p],
-    "odise_copy2d_f32": [c_void_p, c_longlong, c_void_p, c_longlong, c_longlong, c_int, c_float, c_int, c_void_p],
-    "odise_resize_nhwc_f32": [c_void_p, c_longlong, c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_int, c_int,
-                              c_int, c_int, c_void_p],
-    "odise_image_crops_u8_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_image_crops_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_clip_preprocess": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_crop_resize_bicubic": [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_patchify_split_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_nchw_to_nhwc_f32": [c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_void_p],
-    "odise_nhwc_to_nchw_f32": [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_void_p],
-    "odise_attn_mask_bits_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_mha_d32_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
-                          c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_float, c_void_p],
-    "odise_mha_d32_ws_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
-                             c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p],
-    "odise_mask_binarize_f32": [c_void_p, c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_void_p],
-    "odise_pool_normalize_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
-    "odise_l2_normalize_split_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int,
-                                     c_void_p],
-    "odise_class_max_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_void_p],
-    "odise_act_split_f32": [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_void_p],
-    "odise_softmax_split_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int, c_int,
-                                c_float, c_void_p],
-    "odise_upsample_sigmoid_split_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                                         c_int, c_void_p, c_void_p],
-    "odise_query_scores_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                               c_float, c_void_p],
-    "odise_panoptic_inference_f32": [c_void_p] * 9 + [c_int] * 7 + [ctypes.c_double, c_void_p, c_void_p],
-    "odise_instance_inference_f32": [c_void_p] * 9 + [c_int] * 8 + [c_void_p, c_void_p],
-    "odise_postprocess_fused_f32": [c_void_p, c_void_p, c_void_p, c_int] + [c_void_p] * 8 + [ctypes.c_double] + [c_void_p] * 7 +
-                                   [c_int] * 9 + [c_void_p, c_void_p],
-    "odise_set_carveout_policy": [c_int],
-    "odise_set_operand_format": [c_int],
-    "odise_get_operand_format": [],
-    "odise_gather_rows_f32": [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_int, c_void_p, c_longlong, c_longlong,
-                              c_int, c_void_p],
-    "odise_maskclip_preprocess": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    "odise_maskclip_bits_f32": [c_void_p] * 3 + [c_int] * 8 + [c_void_p],
-    "odise_open_vocab_merge_f32": [c_void_p, c_void_p, c_longlong, c_void_p, c_float, c_float, c_void_p, c_void_p, c_int,
-                                   c_int, c_void_p],
-    "odise_attention_tc": [c_void_p, c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p, c_void_p,
-                           c_longlong, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int,
-                           c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p],
-}
 
 
 def load():
@@ -197,26 +84,9 @@ def load():
             f"{_LIB_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` "
             "(odise_b200 has no CPU / eager fallback)")
     lib = ctypes.CDLL(_LIB_PATH)
-    lib.odise_version.restype = c_int
-    lib.odise_launch_count.restype = c_longlong
-    lib.odise_groupnorm_ws_floats.restype = c_longlong
-    lib.odise_groupnorm_ws_floats.argtypes = [c_int, c_int, c_int, c_int]
-    lib.odise_mha_d32_ws_floats.restype = c_longlong
-    lib.odise_panoptic_ws_bytes.restype = c_longlong
-    lib.odise_panoptic_ws_bytes.argtypes = [c_int, c_int, c_int, c_int]
-    lib.odise_instance_ws_bytes.restype = c_longlong
-    lib.odise_instance_ws_bytes.argtypes = [c_int, c_int, c_int, c_int]
-    lib.odise_postprocess_fused_ws_bytes.restype = c_longlong
-    lib.odise_postprocess_fused_ws_bytes.argtypes = [c_int, c_int, c_int, c_int]
-    lib.odise_mha_d32_ws_floats.argtypes = [c_int, c_int, c_int, c_int]
-    for name, args in _SIGS.items():
+    for name, (restype, argtypes) in _PROTOS.items():
         fn = getattr(lib, name)
-        fn.argtypes = args
-        fn.restype = c_int
-    lib.odise_msda_det_workspace_bytes.restype = c_longlong
-    lib.odise_masked_xattn_workspace_bytes.restype = c_longlong
-    lib.odise_mask_loss_workspace_bytes.restype = c_longlong
-    lib.odise_mask_head_workspace_bytes.restype = c_longlong
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = lib
     return lib
 
@@ -244,11 +114,6 @@ def _req(t, dtype, name):
     if t.dtype != dtype:
         raise OdiseError(f"{name}: expected {dtype}, got {t.dtype}")
     return t
-
-
-class PostprocessGeom(ctypes.Structure):
-    """odise_postprocess_geom (include/odise_b200.h): padded size and un-padded image size of sem_seg_postprocess."""
-    _fields_ = [("pad_h", c_int), ("pad_w", c_int), ("img_h", c_int), ("img_w", c_int)]
 
 
 Q8 = "q8"          # value of the engines' `lo` switch in the F16Q8 operand mode (truthy: a second plane exists)

@@ -21,17 +21,19 @@ def _declared():
     return sorted(set(re.findall(r"\b(odise_[a-z0-9_]+)\s*\(", h)))
 
 
-def test_every_declared_symbol_is_exported_and_bound(built):
+def test_every_declared_symbol_is_exported_and_bound_as_declared(built):
     from odise_b200 import lib
     dll = ctypes.CDLL(built)
     names = _declared()
     assert len(names) >= 30
     for n in names:
         assert hasattr(dll, n), f"{n} declared in the header but not exported"
-    bound = set(lib._SIGS) | {"odise_version", "odise_launch_count", "odise_groupnorm_ws_floats", "odise_mha_d32_ws_floats", "odise_panoptic_ws_bytes",
-             "odise_instance_ws_bytes", "odise_postprocess_fused_ws_bytes"}
-    assert set(names) <= bound, set(names) - bound
-    assert lib.load().odise_version() == 100
+    assert set(names) <= set(lib._PROTOS), set(names) - set(lib._PROTOS)     # no prototype skipped by the parser
+    L = lib.load()
+    for n, (restype, argtypes) in lib._PROTOS.items():
+        fn = getattr(L, n)
+        assert fn.restype is restype and list(fn.argtypes) == argtypes, n
+    assert L.odise_version() == 100
 
 
 def test_argument_validation_without_gpu(built):
@@ -94,13 +96,53 @@ def test_auto_split_and_struct_layouts():
     assert lib.auto_split(65536, 320, 2880) == (0, 1) and lib.auto_split(4096, 640, 5760) == (0, 1)
     assert lib.auto_split(256, 1280, 11520)[1] > 1
     assert lib.auto_split(128, 64, 512) == (0, 1)                       # too few k-blocks to split
-    hdr = open(os.path.join(ROOT, "include", "odise_b200.h")).read()
-    m = re.search(r"typedef struct \{([^}]*)\} odise_postprocess_geom;", hdr)
-    fields = [f.strip(" ;") for f in m.group(1).replace("int", "").split(",")]
-    assert fields == [n for n, _ in lib.PostprocessGeom._fields_] and ctypes.sizeof(lib.PostprocessGeom) == 16
+    assert ctypes.sizeof(lib.GemmDesc) == 312 and ctypes.sizeof(lib.PostprocessGeom) == 16
+    assert [n for n, _ in lib.PostprocessGeom._fields_] == ["pad_h", "pad_w", "img_h", "img_w"]
     # the GEMM descriptor mirrors the header field by field
+    hdr = open(os.path.join(ROOT, "include", "odise_b200.h")).read()
     body = re.search(r"typedef struct odise_gemm_desc \{(.*?)\} odise_gemm_desc;", hdr, re.S)
     names = []
     for stmt in re.sub(r"/\*.*?\*/", "", body.group(1), flags=re.S).split(";"):
         names += [re.findall(r"\w+", d)[-1] for d in stmt.split(",") if re.findall(r"\w+", d)]
     assert names == [n for n, _ in lib.GemmDesc._fields_]
+
+
+def test_signatures_bound_from_the_header():
+    """a few entry points typed by hand, so that a wrong mapping rule of lib._parse_header fails here"""
+    from ctypes import c_double, c_float, c_int, c_longlong, c_void_p, POINTER
+    from odise_b200 import lib
+    P = lib._PROTOS
+    assert P["odise_split_f32"] == (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_int,
+                                            c_void_p])
+    assert P["odise_gemm_bf16"] == (c_int, [POINTER(lib.GemmDesc), c_void_p])
+    assert P["odise_postprocess_fused_f32"] == (c_int, [c_void_p] * 3 + [c_int] + [c_void_p] * 8 + [c_double] +
+                                                [c_void_p] * 7 + [c_int] * 9 + [POINTER(lib.PostprocessGeom), c_void_p])
+    assert P["odise_mask_cost_f32"] == (c_int, [c_void_p] * 7 + [c_int] * 9 + [c_float] * 3 + [c_void_p])
+    assert P["odise_msda_det_workspace_bytes"] == (c_longlong, [c_int] * 4)
+    assert P["odise_version"] == (c_int, [])
+
+
+def test_header_parser_refuses_unmapped_types():
+    from ctypes import c_int, c_longlong, c_void_p, POINTER
+    from odise_b200 import lib
+    structs, protos = lib._parse_header("typedef struct { int a, b; size_t* p; } odise_s;  /* odise_y(size_t n); */\n"
+                                        "long long odise_f(const odise_s* s, void* stream);")
+    assert [(n, t) for n, t in structs["odise_s"]._fields_] == [("a", c_int), ("b", c_int), ("p", c_void_p)]
+    assert protos == {"odise_f": (c_longlong, [POINTER(structs["odise_s"]), c_void_p])}
+    with pytest.raises(lib.OdiseError, match="size_t n"):
+        lib._parse_header("int odise_x(size_t n);")
+    with pytest.raises(lib.OdiseError, match="size_t odise_x"):
+        lib._parse_header("size_t odise_x(void);")
+    with pytest.raises(lib.OdiseError, match="size_t b, c"):
+        lib._parse_header("typedef struct { int a; size_t b, c; } odise_s;")
+
+
+def test_constants_match_header_defines():
+    """the ODISE_ACT_* / ODISE_PLANES_* / ODISE_MASK_MAX_* values lib.py spells out, and ODISE_ERR_UNSUPPORTED"""
+    from odise_b200 import lib
+    hdr = open(os.path.join(ROOT, "include", "odise_b200.h")).read()
+    defines = {n: int(v) for n, v in re.findall(r"#define\s+ODISE_(\w+)\s+(\d+)", hdr)}
+    pat = r"(ACT|PLANES|MASK_MAX)_[A-Z0-9_]+"
+    assert {n: getattr(lib, n) for n in dir(lib) if re.fullmatch(pat, n)} == \
+        {n: v for n, v in defines.items() if re.fullmatch(pat, n)}
+    assert lib.ODISE_ERR_UNSUPPORTED == defines["ERR_UNSUPPORTED"]

@@ -221,12 +221,12 @@ NAMES = ["odise_mask_loss_workspace_bytes", "odise_mask_point_sample_u8"] + [
     f"odise_mask_{d}_{s}" for d in ("cost", "loss_forward", "loss_backward", "point_sample") for s in ("f32", "f16", "bf16")]
 
 
-def test_cabi_exports_and_checks(built):
+def test_cabi_exports_prototypes_and_checks(built):
     from odise_b200 import lib
     dll = ctypes.CDLL(built)
     for n in NAMES:
         assert hasattr(dll, n), n
-        assert n in lib._SIGS
+        assert n in lib._PROTOS
     L = lib.load()
     assert L.odise_mask_loss_workspace_bytes(0, 10) == 0
     assert L.odise_mask_loss_workspace_bytes(111, 12544) == 111 * 16 + 111 * 12544 * 8

@@ -207,12 +207,12 @@ NAMES = ["odise_masked_xattn_workspace_bytes"] + [f"odise_masked_xattn_{d}_{s}" 
                                                   for s in ("f32", "f16", "bf16")]
 
 
-def test_cabi_exports_and_checks(built):
+def test_cabi_exports_prototypes_and_checks(built):
     from odise_b200 import lib
     dll = ctypes.CDLL(built)
     for n in NAMES:
         assert hasattr(dll, n), n
-        assert n in lib._SIGS
+        assert n in lib._PROTOS
     L = lib.load()
     ws = L.odise_masked_xattn_workspace_bytes(2, 8, 100, 16384)
     assert ws >= 4 * (2 * 8 * 100 * 34) and ws % 16 == 0

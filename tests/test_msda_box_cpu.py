@@ -19,12 +19,12 @@ def built():
     return ge.build()
 
 
-def test_box_entry_points_are_bound_like_their_twins():
+def test_box_prototypes_match_their_twins():
     """each box entry point takes its 2-column twin's arguments (the f32 forward without out_hi / out_lo)"""
     from odise_b200 import lib
-    assert lib._SIGS["odise_msda_fused_box_f32"] == lib._SIGS["odise_msda_fused_f16"]
+    assert lib._PROTOS["odise_msda_fused_box_f32"][1] == lib._PROTOS["odise_msda_fused_f16"][1]
     for name in FWD[1:] + BWD + DET:
-        assert lib._SIGS[name] == lib._SIGS[name.replace("box_", "")], name
+        assert lib._PROTOS[name][1] == lib._PROTOS[name.replace("box_", "")][1], name
 
 
 @pytest.mark.parametrize("name", FWD + BWD + DET)

@@ -1,6 +1,6 @@
-"""CPU checks of the deterministic MSDeformAttn backward entry points (odise_msda_*_det_*): they are bound in lib._SIGS,
-return ODISE_ERR_ARG / ODISE_ERR_WORKSPACE / ODISE_ERR_UNSUPPORTED without touching a device, and the workspace size
-is the int64 accumulator plus two 8-byte maxima per (image, head)."""
+"""CPU checks of the deterministic MSDeformAttn backward entry points (odise_msda_*_det_*): they are bound from
+lib._PROTOS, return ODISE_ERR_ARG / ODISE_ERR_WORKSPACE / ODISE_ERR_UNSUPPORTED without touching a device, and the
+workspace size is the int64 accumulator plus two 8-byte maxima per (image, head)."""
 import pytest
 import torch
 
@@ -22,15 +22,15 @@ def built():
     return ge.build()
 
 
-def test_bindings_present(built):
+def test_bindings_follow_header_prototypes(built):
     from odise_b200 import lib
     L = lib.load()
     for name, n in TWINS.items():
         default = name.replace("_det", "")
-        assert lib._SIGS[name] == lib._SIGS[default][:-1] + [lib.c_void_p, lib.c_void_p], name
-        assert len(lib._SIGS[name]) == n + 7 + 2
+        assert lib._PROTOS[name][1] == lib._PROTOS[default][1][:-1] + [lib.c_void_p, lib.c_void_p], name
+        assert len(lib._PROTOS[name][1]) == n + 7 + 2
         assert getattr(L, name).restype is lib.c_int
-    assert "odise_msda_det_workspace_bytes" in lib._SIGS
+    assert "odise_msda_det_workspace_bytes" in lib._PROTOS
     assert L.odise_msda_det_workspace_bytes.restype is lib.c_longlong
 
 
