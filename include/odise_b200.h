@@ -602,6 +602,58 @@ int odise_fpn_upsample_add_backward_f32(const float* grad_y, float* grad_z, long
                                         int C, int h, int w, int H, int W, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Category scoring for training (odise.py:181-207 CategoryODISE.cal_pred_logits with helper.py:79-109
+ * ensemble_logits_with_labels(..., "max")): mask_embed [R, C] (R = B * Q rows), text_embed [Kp, C], null_embed [1, C],
+ * logit_scale a float32 scalar on the device, group_start int32 [K + 1] on the device: class k's prompts are
+ * [group_start[k], group_start[k + 1]), group_start[0] = 0, group_start[K] = Kp, every group 1..255 prompts (not
+ * checked: the table is not read on the host).  All tensors contiguous.  _f32 / _f16 / _bf16: mask_embed, logits and
+ * their gradients in float, __half or __nv_bfloat16; text_embed, null_embed and their gradients in the same type, or
+ * in float when bank_f32 = 1 (a float32 bank under autocast; ignored by _f32).  All arithmetic fp32.
+ * odise_category_logits_forward_*: with ^ = x / max(|x|, 1e-12) per row (F.normalize), s_rj = scale <m^_r, t^_j>:
+ *   logits [R, K + 1] = the max of s_rj over class k's prompts, and s against n^ in column K.  In 16 bits m^, t^, n^,
+ *   the dot product and scale are rounded to the storage type where torch's autocast rounds them, and the product is
+ *   rounded once.  Among equal stored values the lowest prompt index wins; a NaN wins over every number (torch's
+ *   max(dim)).  winners uint8 [R, K + 1] = the winning prompt's offset in its group (0 in column K); norms float32
+ *   [R + Kp + 1] = the clamped norms max(|x|, 1e-12) of the mask rows, the prompts and the null row.
+ * odise_category_logits_backward_*: from the forward's inputs, winners, norms and grad_logits [R, K + 1]:
+ *   grad_mask_embed [R, C], grad_text_embed [Kp, C], grad_null_embed [1, C] (each gradient routed to the prompt the
+ *   forward chose, then through the normalization) and grad_logit_scale, one float32 (= sum grad_logits * s / scale).
+ *   workspace: odise_category_logits_workspace_bytes(R, C, K, Kp) bytes, 4-byte aligned, any content (0 for shapes the
+ *   entry points refuse); it holds fp32 partials over fixed row splits summed in split order, without atomics, so every
+ *   gradient is bit-reproducible.
+ * Limits: C a multiple of 32 up to 768, 1 <= K <= Kp <= 2048, R * (K + 1) and R * C < 2^31 (ODISE_ERR_UNSUPPORTED
+ * otherwise).  The forward is one launch, the backward three.  No host synchronisation and no allocation (CUDA-graph
+ * capturable). */
+long long odise_category_logits_workspace_bytes(int R, int C, int K, int Kp);
+int odise_category_logits_forward_f32(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                      const float* logit_scale, const int32_t* group_start, void* logits,
+                                      uint8_t* winners, float* norms, int R, int C, int K, int Kp, int bank_f32,
+                                      void* stream);
+int odise_category_logits_forward_f16(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                      const float* logit_scale, const int32_t* group_start, void* logits,
+                                      uint8_t* winners, float* norms, int R, int C, int K, int Kp, int bank_f32,
+                                      void* stream);
+int odise_category_logits_forward_bf16(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                       const float* logit_scale, const int32_t* group_start, void* logits,
+                                       uint8_t* winners, float* norms, int R, int C, int K, int Kp, int bank_f32,
+                                       void* stream);
+int odise_category_logits_backward_f32(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                       const float* logit_scale, const int32_t* group_start, const uint8_t* winners,
+                                       const float* norms, const void* grad_logits, void* grad_mask_embed,
+                                       void* grad_text_embed, void* grad_null_embed, float* grad_logit_scale, int R,
+                                       int C, int K, int Kp, int bank_f32, void* workspace, void* stream);
+int odise_category_logits_backward_f16(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                       const float* logit_scale, const int32_t* group_start, const uint8_t* winners,
+                                       const float* norms, const void* grad_logits, void* grad_mask_embed,
+                                       void* grad_text_embed, void* grad_null_embed, float* grad_logit_scale, int R,
+                                       int C, int K, int Kp, int bank_f32, void* workspace, void* stream);
+int odise_category_logits_backward_bf16(const void* mask_embed, const void* text_embed, const void* null_embed,
+                                        const float* logit_scale, const int32_t* group_start, const uint8_t* winners,
+                                        const float* norms, const void* grad_logits, void* grad_mask_embed,
+                                        void* grad_text_embed, void* grad_null_embed, float* grad_logit_scale, int R,
+                                        int C, int K, int Kp, int bank_f32, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

@@ -937,6 +937,92 @@ def mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_p
     return ge, gx
 
 
+# the category-scoring kernels' limits: C a multiple of 32 up to 768, up to 2048 prompts, groups of 1..255 prompts
+CATEGORY_C_MULTIPLE, CATEGORY_MAX_C, CATEGORY_MAX_PROMPTS, CATEGORY_MAX_GROUP = 32, 768, 2048, 255
+
+
+def _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start, winners=None, norms=None,
+                     grad_logits=None):
+    """Checks of the category-scoring entry points, without data and without the library (the fake implementations of
+    odise_b200.category's ops call it too): mask_embed [B, Q, C] float32 / float16 / bfloat16, text_embed [Kp, C] and
+    null_embed [1, C] of mask_embed's dtype or (16-bit mask_embed only) both float32, logit_scale a float32 scalar,
+    group_start int32 [K + 1], all contiguous CUDA tensors; for the backward winners uint8 and grad_logits of
+    mask_embed's dtype [B, Q, K + 1], norms float32 [B*Q + Kp + 1].  -> (suffix, bank_f32, B, Q, C, K, Kp)"""
+    if mask_embed.dtype not in _XATTN_SFX:
+        raise OdiseError(f"mask_embed: expected float32, float16 or bfloat16, got {mask_embed.dtype}")
+    if mask_embed.dim() != 3 or text_embed.dim() != 2 or group_start.dim() != 1:
+        raise OdiseError(f"mask_embed must be [B, Q, C], text_embed [Kp, C] and group_start [K + 1], got "
+                         f"{tuple(mask_embed.shape)}, {tuple(text_embed.shape)} and {tuple(group_start.shape)}")
+    B, Q, C = mask_embed.shape
+    Kp, K = text_embed.shape[0], group_start.shape[0] - 1
+    if min(B, Q) <= 0 or C % CATEGORY_C_MULTIPLE or not 0 < C <= CATEGORY_MAX_C or not 1 <= K <= Kp \
+            or Kp > CATEGORY_MAX_PROMPTS or B * Q * max(K + 1, C) >= 2 ** 31:
+        raise OdiseError(f"category scoring: B = {B}, Q = {Q}, C = {C}, K = {K}, Kp = {Kp} not supported (C a multiple "
+                         f"of {CATEGORY_C_MULTIPLE} up to {CATEGORY_MAX_C}, 1 <= K <= Kp <= {CATEGORY_MAX_PROMPTS})")
+    bank = text_embed.dtype
+    if bank != mask_embed.dtype and not (bank == torch.float32 and mask_embed.dtype != torch.float32):
+        raise OdiseError(f"text_embed: expected {mask_embed.dtype} or (16-bit mask_embed) float32, got {bank}")
+    _req_shape(mask_embed, mask_embed.dtype, (B, Q, C), "mask_embed")
+    _req_shape(text_embed, bank, (Kp, C), "text_embed")
+    _req_shape(null_embed, bank, (1, C), "null_embed")
+    _req_shape(logit_scale, torch.float32, (), "logit_scale")
+    _req_shape(group_start, torch.int32, (K + 1,), "group_start")
+    if winners is not None:
+        _req_shape(winners, torch.uint8, (B, Q, K + 1), "winners")
+    if norms is not None:
+        _req_shape(norms, torch.float32, (B * Q + Kp + 1,), "norms")
+    if grad_logits is not None:
+        _req_shape(grad_logits, mask_embed.dtype, (B, Q, K + 1), "grad_logits")
+    return _XATTN_SFX[mask_embed.dtype], int(bank != mask_embed.dtype), B, Q, C, K, Kp
+
+
+def category_group_start(sizes):
+    """group_start of the category-scoring kernels, as Python ints, for the classes' prompt counts (each 1..255)"""
+    if not sizes or min(sizes) < 1 or max(sizes) > CATEGORY_MAX_GROUP:
+        raise OdiseError(f"category scoring: groups of 1..{CATEGORY_MAX_GROUP} prompts, got sizes from "
+                         f"{min(sizes, default=None)} to {max(sizes, default=None)}")
+    out = [0]
+    for n in sizes:
+        out.append(out[-1] + n)
+    return out
+
+
+def category_logits_forward(mask_embed, text_embed, null_embed, logit_scale, group_start):
+    """CategoryODISE.cal_pred_logits with the "max" ensemble (odise_category_logits_forward_* by mask_embed's dtype):
+    -> (logits [B, Q, K + 1] in mask_embed's dtype, winners uint8 [B, Q, K + 1] = each max's prompt offset in its
+    group, norms float32 [B*Q + Kp + 1] = the clamped row norms of mask_embed, text_embed and null_embed).  group_start
+    int32 [K + 1] on the device holds the classes' prompt offsets (category_group_start); it is not read on the host.
+    OdiseError on CPU, non-contiguous or mixed-dtype tensors and on shapes the kernels do not take."""
+    sfx, bank_f32, B, Q, C, K, Kp = _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start)
+    dev = mask_embed.device
+    out = torch.empty(B, Q, K + 1, dtype=mask_embed.dtype, device=dev)
+    win = torch.empty(B, Q, K + 1, dtype=torch.uint8, device=dev)
+    norms = torch.empty(B * Q + Kp + 1, dtype=torch.float32, device=dev)
+    fn = "odise_category_logits_forward_" + sfx
+    _check(getattr(load(), fn)(_ptr(mask_embed), _ptr(text_embed), _ptr(null_embed), _ptr(logit_scale),
+                               _ptr(group_start), _ptr(out), _ptr(win), _ptr(norms), B * Q, C, K, Kp, bank_f32,
+                               _stream()), fn)
+    return out, win, norms
+
+
+def category_logits_backward(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms,
+                             grad_logits):
+    """Backward of category_logits_forward (odise_category_logits_backward_*) -> (grad_mask_embed, grad_text_embed,
+    grad_null_embed, grad_logit_scale): each in its input's dtype, the scale's a float32 scalar.  Each gradient goes to
+    the prompt the forward chose; fixed-order sums without atomics, so every gradient is bit-reproducible."""
+    sfx, bank_f32, B, Q, C, K, Kp = _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start,
+                                                     winners, norms, grad_logits)
+    gm, gt, gn = torch.empty_like(mask_embed), torch.empty_like(text_embed), torch.empty_like(null_embed)
+    gs = torch.empty((), dtype=torch.float32, device=mask_embed.device)
+    ws = torch.empty(int(load().odise_category_logits_workspace_bytes(B * Q, C, K, Kp)), dtype=torch.uint8,
+                     device=mask_embed.device)
+    fn = "odise_category_logits_backward_" + sfx
+    _check(getattr(load(), fn)(_ptr(mask_embed), _ptr(text_embed), _ptr(null_embed), _ptr(logit_scale),
+                               _ptr(group_start), _ptr(winners), _ptr(norms), _ptr(grad_logits), _ptr(gm), _ptr(gt),
+                               _ptr(gn), _ptr(gs), B * Q, C, K, Kp, bank_f32, _ptr(ws), _stream()), fn)
+    return gm, gt, gn, gs
+
+
 FPN_C_MULTIPLE = 32     # the FPN upsample-add kernels take C a multiple of this
 
 
