@@ -29,7 +29,6 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from . import lib
-from . import msda as _msda  # noqa: F401  (holds the "DEF" library of the odise_b200 namespace; defined first)
 
 _OPS = torch.library.Library("odise_b200", "FRAGMENT")
 _OPS.define("category_logits(Tensor mask_embed, Tensor text_embed, Tensor null_embed, Tensor logit_scale, "

@@ -380,67 +380,24 @@ extern "C" long long odise_category_logits_workspace_bytes(int R, int C, int K, 
   return ((long long)ob::cl_splits(R) * (Kp + 1) * C + (long long)R * C + R) * (long long)sizeof(float);
 }
 
-extern "C" int odise_category_logits_forward_f32(const void* mask_embed, const void* text_embed,
-                                                 const void* null_embed, const float* logit_scale,
-                                                 const int32_t* group_start, void* logits, uint8_t* winners,
-                                                 float* norms, int R, int C, int K, int Kp, int bank_f32,
-                                                 void* stream) {
-  (void)bank_f32;
-  return ob::cl_forward<float, float>(mask_embed, text_embed, null_embed, logit_scale, group_start, logits, winners,
-                                      norms, R, C, K, Kp, stream);
-}
-
-extern "C" int odise_category_logits_forward_f16(const void* mask_embed, const void* text_embed,
-                                                 const void* null_embed, const float* logit_scale,
-                                                 const int32_t* group_start, void* logits, uint8_t* winners,
-                                                 float* norms, int R, int C, int K, int Kp, int bank_f32,
-                                                 void* stream) {
-  auto fn = bank_f32 ? ob::cl_forward<__half, float> : ob::cl_forward<__half, __half>;
-  return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, logits, winners, norms, R, C, K, Kp, stream);
-}
-
-extern "C" int odise_category_logits_forward_bf16(const void* mask_embed, const void* text_embed,
-                                                  const void* null_embed, const float* logit_scale,
-                                                  const int32_t* group_start, void* logits, uint8_t* winners,
-                                                  float* norms, int R, int C, int K, int Kp, int bank_f32,
-                                                  void* stream) {
-  auto fn = bank_f32 ? ob::cl_forward<__nv_bfloat16, float> : ob::cl_forward<__nv_bfloat16, __nv_bfloat16>;
-  return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, logits, winners, norms, R, C, K, Kp, stream);
-}
-
-extern "C" int odise_category_logits_backward_f32(const void* mask_embed, const void* text_embed,
-                                                  const void* null_embed, const float* logit_scale,
-                                                  const int32_t* group_start, const uint8_t* winners,
-                                                  const float* norms, const void* grad_logits, void* grad_mask_embed,
-                                                  void* grad_text_embed, void* grad_null_embed,
-                                                  float* grad_logit_scale, int R, int C, int K, int Kp, int bank_f32,
-                                                  void* workspace, void* stream) {
-  (void)bank_f32;
-  return ob::cl_backward<float, float>(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms,
-                                       grad_logits, grad_mask_embed, grad_text_embed, grad_null_embed,
-                                       grad_logit_scale, R, C, K, Kp, workspace, stream);
-}
-
-extern "C" int odise_category_logits_backward_f16(const void* mask_embed, const void* text_embed,
-                                                  const void* null_embed, const float* logit_scale,
-                                                  const int32_t* group_start, const uint8_t* winners,
-                                                  const float* norms, const void* grad_logits, void* grad_mask_embed,
-                                                  void* grad_text_embed, void* grad_null_embed,
-                                                  float* grad_logit_scale, int R, int C, int K, int Kp, int bank_f32,
-                                                  void* workspace, void* stream) {
-  auto fn = bank_f32 ? ob::cl_backward<__half, float> : ob::cl_backward<__half, __half>;
-  return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits,
-            grad_mask_embed, grad_text_embed, grad_null_embed, grad_logit_scale, R, C, K, Kp, workspace, stream);
-}
-
-extern "C" int odise_category_logits_backward_bf16(const void* mask_embed, const void* text_embed,
-                                                   const void* null_embed, const float* logit_scale,
-                                                   const int32_t* group_start, const uint8_t* winners,
-                                                   const float* norms, const void* grad_logits,
-                                                   void* grad_mask_embed, void* grad_text_embed,
-                                                   void* grad_null_embed, float* grad_logit_scale, int R, int C, int K,
-                                                   int Kp, int bank_f32, void* workspace, void* stream) {
-  auto fn = bank_f32 ? ob::cl_backward<__nv_bfloat16, float> : ob::cl_backward<__nv_bfloat16, __nv_bfloat16>;
-  return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits,
-            grad_mask_embed, grad_text_embed, grad_null_embed, grad_logit_scale, R, C, K, Kp, workspace, stream);
-}
+#define CL_ENTRY(sfx, T)                                                                                               \
+  extern "C" int odise_category_logits_forward_##sfx(                                                                  \
+      const void* mask_embed, const void* text_embed, const void* null_embed, const float* logit_scale,                \
+      const int32_t* group_start, void* logits, uint8_t* winners, float* norms, int R, int C, int K, int Kp,           \
+      int bank_f32, void* stream) {                                                                                    \
+    auto fn = bank_f32 ? ob::cl_forward<T, float> : ob::cl_forward<T, T>;                                              \
+    return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, logits, winners, norms, R, C, K, Kp,       \
+              stream);                                                                                                 \
+  }                                                                                                                    \
+  extern "C" int odise_category_logits_backward_##sfx(                                                                 \
+      const void* mask_embed, const void* text_embed, const void* null_embed, const float* logit_scale,                \
+      const int32_t* group_start, const uint8_t* winners, const float* norms, const void* grad_logits,                 \
+      void* grad_mask_embed, void* grad_text_embed, void* grad_null_embed, float* grad_logit_scale, int R, int C,      \
+      int K, int Kp, int bank_f32, void* workspace, void* stream) {                                                    \
+    auto fn = bank_f32 ? ob::cl_backward<T, float> : ob::cl_backward<T, T>;                                            \
+    return fn(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits,               \
+              grad_mask_embed, grad_text_embed, grad_null_embed, grad_logit_scale, R, C, K, Kp, workspace, stream);    \
+  }
+CL_ENTRY(f32, float)
+CL_ENTRY(f16, __half)
+CL_ENTRY(bf16, __nv_bfloat16)

@@ -31,7 +31,6 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from . import lib
-from . import msda as _msda  # noqa: F401  (holds the "DEF" library of the odise_b200 namespace; defined first)
 from .masked_attn import CrossAttentionLayer, _activation
 
 _OPS = torch.library.Library("odise_b200", "FRAGMENT")

@@ -108,12 +108,36 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _req(t, dtype, name):
+def _launch(name, *args):
+    """Run entry point `name` with args on the current stream; OdiseError if it returns an error code."""
+    _check(getattr(load(), name)(*args, _stream()), name)
+
+
+# the entry-point suffix of each storage dtype (bool masks are read as bytes); each wrapper states which dtypes it takes
+_SFX = {torch.float32: "f32", torch.float64: "f64", torch.float16: "f16", torch.bfloat16: "bf16", torch.uint8: "u8",
+        torch.bool: "u8"}
+_FLOATS = (torch.float32, torch.float16, torch.bfloat16)     # the storage types of the training kernels
+
+
+def _tensor(t, name, dtypes, shape=None, contiguous=True):
+    """Raise OdiseError unless t is a CUDA tensor of `dtypes` (one dtype or a tuple), contiguous (unless
+    contiguous=False: strided operands) and, if given, of `shape`.  Reads no data, so the fake implementations of the
+    custom ops check with it too."""
+    dtypes = dtypes if isinstance(dtypes, tuple) else (dtypes,)
     if not t.is_cuda:
-        raise OdiseError(f"{name}: expected a CUDA tensor (odise_b200 kernels only run on the GPU)")
-    if t.dtype != dtype:
-        raise OdiseError(f"{name}: expected {dtype}, got {t.dtype}")
-    return t
+        raise OdiseError(f"{name} must be a CUDA tensor")
+    if t.dtype not in dtypes:
+        raise OdiseError(f"{name}: expected {' or '.join(str(d)[6:] for d in dtypes)}, got {t.dtype}")
+    if contiguous and not t.is_contiguous():
+        raise OdiseError(f"{name} tensor has to be contiguous")
+    if shape is not None and t.shape != shape:
+        raise OdiseError(f"{name}: expected shape {shape}, got {tuple(t.shape)}")
+
+
+def _scratch(nbytes, device):
+    """One call's device scratch of nbytes from torch's allocator (stream-ordered, and private to a captured CUDA
+    graph).  Unlike workspace() it is never shared: mask_loss_forward returns its buffer as the backward's state."""
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
 
 
 Q8 = "q8"          # value of the engines' `lo` switch in the F16Q8 operand mode (truthy: a second plane exists)
@@ -231,7 +255,7 @@ class GnStats:
 
 def split(x, out=None, lo=True, f16=False):
     """fp32 [rows, cols] (last dim contiguous) -> Planes (bf16 pair; f16=True: fp16 pair; lo=lib.Q8: F16Q8)."""
-    _req(x, torch.float32, "x")
+    _tensor(x, "x", torch.float32, contiguous=False)
     x2 = x.reshape(-1, x.shape[-1])
     rows, cols = x2.shape
     assert x2.stride(1) == 1
@@ -365,62 +389,49 @@ def gemm_tile_policy(M, N, K, batch=1, conv=False, nmma=2):
     return bn.value, bool(pair.value)
 
 
-def msda_forward(value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step=128):
-    """Drop-in for MSDA.ms_deform_attn_forward (reference ops/src/vision.cpp:19): same arguments, same result
-    shape [N, Lq, M*D], same error behaviour class (RuntimeError on non-contiguous / non-CUDA input)."""
-    for t, nm in ((value, "value"), (sampling_locations, "sampling_loc"), (attention_weights, "attn_weight")):
-        if not t.is_cuda:
-            raise OdiseError(f"{nm} must be a CUDA tensor")  # reference: AT_ERROR("Not implemented on the CPU")
-        if not t.is_contiguous():
-            raise OdiseError(f"{nm} tensor has to be contiguous")  # reference .cu:33-37
-        _req(t, torch.float32, nm)
+def _msda_inputs(tensors, im2col_step, dtypes=(torch.float32, torch.float64)):
+    """Checks of ms_deform_attn_cuda_forward / _backward (reference .cu:33-57, :98-121) for the float / double entry
+    points: CUDA, contiguous, all of value's dtype, one of `dtypes`, batch divisible by min(batch, im2col_step).
+    -> the entry points' dtype suffix"""
+    (value, _), *rest = tensors
+    _tensor(value, "value", dtypes)
+    for t, nm in rest:
+        _tensor(t, nm, value.dtype)
+    N = value.shape[0]
+    step = min(N, im2col_step)
+    if step <= 0 or N % step != 0:
+        raise OdiseError(f"batch({N}) must divide im2col_step({step})")  # reference .cu:57
+    return _SFX[value.dtype]
+
+
+def _msda_index(device, spatial_shapes, level_start_index):
+    """spatial_shapes and level_start_index as the MSDA kernels read them: contiguous int64 on the value's device"""
+    return [t.to(device=device, dtype=torch.int64).contiguous() for t in (spatial_shapes, level_start_index)]
+
+
+def _msda_forward(dtypes, value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step):
+    sfx = _msda_inputs(((value, "value"), (sampling_locations, "sampling_loc"), (attention_weights, "attn_weight")),
+                       im2col_step, dtypes)
     N, S, M, D = value.shape
     _, Lq, _, L, P, _ = sampling_locations.shape
-    step = min(N, im2col_step)
-    if N % step != 0:
-        raise OdiseError(f"batch({N}) must divide im2col_step({step})")  # reference .cu:57
-    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
-    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
-    out = torch.empty(N, Lq, M * D, dtype=torch.float32, device=value.device)
-    _check(load().odise_msda_forward_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_locations),
-                                         _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P, _stream()),
-           "odise_msda_forward_f32")
+    ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
+    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
+    _launch("odise_msda_forward_" + sfx, _ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_locations),
+            _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P)
     return out
 
 
-def _msda_inputs(tensors, im2col_step):
-    """Checks of ms_deform_attn_cuda_forward / _backward (reference .cu:33-57, :98-121) for the float / double entry
-    points: CUDA, contiguous, one floating dtype (float32 or float64), batch divisible by min(batch, im2col_step)."""
-    dtype = tensors[0][0].dtype
-    if dtype not in (torch.float32, torch.float64):
-        raise OdiseError(f"value: expected float32 or float64, got {dtype}")
-    for t, nm in tensors:
-        if not t.is_cuda:
-            raise OdiseError(f"{nm} must be a CUDA tensor")
-        if not t.is_contiguous():
-            raise OdiseError(f"{nm} tensor has to be contiguous")
-        _req(t, dtype, nm)
-    N = tensors[0][0].shape[0]
-    step = min(N, im2col_step)
-    if step <= 0 or N % step != 0:
-        raise OdiseError(f"batch({N}) must divide im2col_step({step})")
-    return dtype
+def msda_forward(value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step=128):
+    """Drop-in for MSDA.ms_deform_attn_forward (reference ops/src/vision.cpp:19): same arguments, same result
+    shape [N, Lq, M*D], same error behaviour class (RuntimeError on non-contiguous / non-CUDA input).  float32."""
+    return _msda_forward(torch.float32, value, spatial_shapes, level_start_index, sampling_locations,
+                         attention_weights, im2col_step)
 
 
 def msda_forward_f64(value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step=128):
     """msda_forward in float64 (the reference's AT_DISPATCH_FLOATING_TYPES double instantiation)."""
-    _msda_inputs(((value, "value"), (sampling_locations, "sampling_loc"), (attention_weights, "attn_weight")),
-                 im2col_step)
-    _req(value, torch.float64, "value")
-    N, S, M, D = value.shape
-    _, Lq, _, L, P, _ = sampling_locations.shape
-    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
-    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
-    out = torch.empty(N, Lq, M * D, dtype=torch.float64, device=value.device)
-    _check(load().odise_msda_forward_f64(_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_locations),
-                                         _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P, _stream()),
-           "odise_msda_forward_f64")
-    return out
+    return _msda_forward(torch.float64, value, spatial_shapes, level_start_index, sampling_locations,
+                         attention_weights, im2col_step)
 
 
 def _msda_backward_shapes(value, sampling_loc, grad_output):
@@ -433,11 +444,6 @@ def _msda_backward_shapes(value, sampling_loc, grad_output):
     return N, S, M, D, L, Lq, P
 
 
-def _msda_det_workspace(N, S, M, D, device):
-    """workspace of the deterministic backward entry points (odise_msda_det_workspace_bytes), from torch's allocator"""
-    return torch.empty(int(load().odise_msda_det_workspace_bytes(N, S, M, D)), dtype=torch.uint8, device=device)
-
-
 def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=128,
                   *, deterministic=False):
     """Drop-in for MSDA.ms_deform_attn_backward (reference ops/src/vision.cpp:20): same arguments, returns
@@ -446,82 +452,100 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     min(batch, im2col_step) does not divide.  The whole batch is one launch (im2col_step only checked).
     deterministic=True runs odise_msda_backward_det_f32 / _f64: grad_value summed in int64 fixed point, so its bits depend
     on the inputs only (include/odise_b200.h states the error bound); the other two results are the same bits."""
-    dtype = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
-                          (grad_output, "grad_output")), im2col_step)
+    sfx = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
+                        (grad_output, "grad_output")), im2col_step)
     N, S, M, D, L, Lq, P = _msda_backward_shapes(value, sampling_loc, grad_output)
-    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
-    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
+    ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
     grad_value = torch.empty_like(value)
     grad_loc = torch.empty_like(sampling_loc)
     grad_attn = torch.empty_like(attn_weight)
-    sfx = "f32" if dtype == torch.float32 else "f64"
     args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output), _ptr(grad_value),
             _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P)
     if deterministic:
-        ws = _msda_det_workspace(N, S, M, D, value.device)
-        fn = "odise_msda_backward_det_" + sfx
-        _check(getattr(load(), fn)(*args, _ptr(ws), _stream()), fn)
+        ws = _scratch(load().odise_msda_det_workspace_bytes(N, S, M, D), value.device)
+        _launch("odise_msda_backward_det_" + sfx, *args, _ptr(ws))
     else:
-        fn = "odise_msda_backward_" + sfx
-        _check(getattr(load(), fn)(*args, _stream()), fn)
+        _launch("odise_msda_backward_" + sfx, *args)
     return [grad_value, grad_loc, grad_attn]
 
 
 ODISE_ERR_UNSUPPORTED = 10006
 
 
-def _msda_d32_only(fn, S, M, D, L, P):
-    """The shapes the fused backward, the 16-bit fused forward and every box entry point take (d32_ok in msda.cu; their
-    entry points return ODISE_ERR_UNSUPPORTED on any other): D = 32, L*P <= 32 and S*M*D < 2^31.  Raises before any
-    launch, and needs no library, so that the fake implementations of odise_b200.msda's ops refuse the same shapes."""
-    if not (D == 32 and L * P <= 32 and S * M * D < 2 ** 31):
-        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
+def _msda_box(reference_points):
+    """True for box reference points [N, Lq, L, 4] (cx, cy, w, h): the odise_msda_fused_box_* entry points."""
+    return reference_points.dim() == 4 and reference_points.shape[-1] == 4
 
 
-def _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
-                       dtype=torch.float32):
-    """Checks of the fused entry points: CUDA, contiguous, reference_points float32 and every other tensor of `dtype`,
-    and the layouts of odise_msda_fused_f32 (value [N, S, M, D], reference_points [N, Lq, L, 2] or boxes [N, Lq, L, 4]
-    with a storage offset that keeps them 16-byte aligned, offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P],
-    grad_output [N, Lq, M*D]).  -> (N, S, M, D, L, Lq, P,
-    spatial_shapes, level_start_index) with the two index tensors as int64 on the value's device."""
-    named = [(value, "value"), (reference_points, "reference_points"), (offsets, "offsets"), (logits, "logits")]
-    if grad_output is not None:
-        named.append((grad_output, "grad_output"))
-    for t, nm in named:
-        if not t.is_cuda:
-            raise OdiseError(f"{nm} must be a CUDA tensor")
-        if not t.is_contiguous():
-            raise OdiseError(f"{nm} tensor has to be contiguous")
-        _req(t, torch.float32 if nm == "reference_points" else dtype, nm)
+def _msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
+                     deterministic=False, dtypes=_FLOATS):
+    """Checks of a fused MSDA call, the forward or (grad_output given) the backward, without data and without the
+    library (the fake implementations of odise_b200.msda's ops call it too): CUDA, contiguous, value of one of `dtypes`
+    and offsets, logits and grad_output of its dtype, reference_points float32, in the layouts of odise_msda_fused_f32
+    (value [N, S, M, D], reference_points [N, Lq, L, 2] or boxes [N, Lq, L, 4] with a storage offset that keeps them
+    16-byte aligned, offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P], grad_output [N, Lq, M*D]).  The 16-bit, the
+    box and every backward entry point take D = 32, L*P <= 32 and S*M*D < 2^31 only (d32_ok in msda.cu; they return
+    ODISE_ERR_UNSUPPORTED on any other): such shapes raise here, before any launch.
+    -> (entry point, N, S, M, D, L, Lq, P)"""
+    _tensor(value, "value", dtypes)
     if value.dim() != 4 or offsets.dim() != 6:
         raise OdiseError(f"value must be [N, S, M, D] and offsets [N, Lq, M, L, P, 2], got {tuple(value.shape)} and "
                          f"{tuple(offsets.shape)}")
     N, S, M, D = value.shape
     _, Lq, _, L, P, _ = offsets.shape
-    rw = 4 if _msda_box(reference_points) else 2
-    want = {"offsets": (N, Lq, M, L, P, 2), "reference_points": (N, Lq, L, rw), "logits": (N, Lq, M, L * P),
-            "spatial_shapes": (L, 2), "level_start_index": (L,)}
+    box = _msda_box(reference_points)
+    _tensor(reference_points, "reference_points", torch.float32, (N, Lq, L, 4 if box else 2))
+    _tensor(offsets, "offsets", value.dtype, (N, Lq, M, L, P, 2))
+    _tensor(logits, "logits", value.dtype, (N, Lq, M, L * P))
     if grad_output is not None:
-        want["grad_output"] = (N, Lq, M * D)
-    for t, nm in named[1:] + [(spatial_shapes, "spatial_shapes"), (level_start_index, "level_start_index")]:
-        if tuple(t.shape) != want[nm]:
-            alt = f" or {want[nm][:3] + (4,)}" if nm == "reference_points" else ""
-            raise OdiseError(f"{nm}: expected shape {want[nm]}{alt}, got {tuple(t.shape)}")
-    if rw == 4 and reference_points.storage_offset() % 4:
+        _tensor(grad_output, "grad_output", value.dtype, (N, Lq, M * D))
+    for t, nm, want in ((spatial_shapes, "spatial_shapes", (L, 2)), (level_start_index, "level_start_index", (L,))):
+        if t.shape != want:
+            raise OdiseError(f"{nm}: expected shape {want}, got {tuple(t.shape)}")
+    if box and reference_points.storage_offset() % 4:
         # a box is one 16-byte load (the entry points return ODISE_ERR_ARG otherwise); checked on the storage offset,
         # which a fake tensor has too, so that a view into an allocation fails here and not at the launch
         raise OdiseError("reference_points: box reference points must start 16 bytes into their storage "
                          f"(storage offset a multiple of 4 floats, got {reference_points.storage_offset()}); pass a "
                          "copy")
-    ss = spatial_shapes.to(device=value.device, dtype=torch.int64).contiguous()
-    ls = level_start_index.to(device=value.device, dtype=torch.int64).contiguous()
-    return N, S, M, D, L, Lq, P, ss, ls
+    fn = (f"odise_msda_fused_{'box_' if box else ''}{'' if grad_output is None else 'backward_'}"
+          f"{'det_' if deterministic else ''}{_SFX[value.dtype]}")
+    d32_only = box or grad_output is not None or value.dtype != torch.float32
+    if d32_only and not (D == 32 and L * P <= 32 and S * M * D < 2 ** 31):
+        raise OdiseError(f"{fn}: D = {D}, L*P = {L * P} not supported (D = 32, L*P <= 32 and S*M*D < 2^31 only)")
+    return fn, N, S, M, D, L, Lq, P
 
 
-def _msda_box(reference_points):
-    """True for box reference points [N, Lq, L, 4] (cx, cy, w, h): the odise_msda_fused_box_* entry points."""
-    return reference_points.dim() == 4 and reference_points.shape[-1] == 4
+def _msda_fused_forward(dtypes, value, spatial_shapes, level_start_index, reference_points, offsets, logits):
+    fn, N, S, M, D, L, Lq, P = _msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets,
+                                                logits, dtypes=dtypes)
+    ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
+    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
+    planes = (None, None) if fn == "odise_msda_fused_f32" else ()    # its out_hi / out_lo, which only the engines use
+    _launch(fn, _ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(out),
+            *planes, N, S, M, D, L, Lq, P)
+    return out
+
+
+def _msda_fused_backward(dtypes, value, spatial_shapes, level_start_index, reference_points, offsets, logits,
+                         grad_output, deterministic):
+    fn, N, S, M, D, L, Lq, P = _msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets,
+                                                logits, grad_output, deterministic, dtypes)
+    ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
+    # the default 16-bit entry points accumulate grad_value in a float32 buffer, rounded once below
+    grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
+    grad_offs = torch.empty_like(offsets)
+    grad_logits = torch.empty_like(logits)
+    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
+            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
+    if deterministic:
+        ws = _scratch(load().odise_msda_det_workspace_bytes(N, S, M, D), value.device)
+        _launch(fn, *args, _ptr(ws))
+    else:
+        _launch(fn, *args)
+    if grad_value.dtype != value.dtype:
+        grad_value = grad_value.to(value.dtype)
+    return grad_value, grad_offs, grad_logits
 
 
 def msda_fused_forward(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
@@ -530,19 +554,8 @@ def msda_fused_forward(value, spatial_shapes, level_start_index, reference_point
     take odise_msda_fused_box_f32 (loc = ref.xy + off / P * ref.wh * 0.5), D = 32, L*P <= 32 and S*M*D < 2^31 only.
     RuntimeError on CPU, non-contiguous or non-float32 tensors, on shapes that disagree and on a D the kernel does not
     take."""
-    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
-                                                      offsets, logits)
-    out = torch.empty(N, Lq, M * D, dtype=torch.float32, device=value.device)
-    if _msda_box(reference_points):
-        fn = "odise_msda_fused_box_f32"
-        _msda_d32_only(fn, S, M, D, L, P)
-        _check(load().odise_msda_fused_box_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
-                                               _ptr(logits), _ptr(out), N, S, M, D, L, Lq, P, _stream()), fn)
-        return out
-    _check(load().odise_msda_fused_f32(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets),
-                                       _ptr(logits), _ptr(out), None, None, N, S, M, D, L, Lq, P, _stream()),
-           "odise_msda_fused_f32")
-    return out
+    return _msda_fused_forward(torch.float32, value, spatial_shapes, level_start_index, reference_points, offsets,
+                               logits)
 
 
 def msda_fused_backward(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output, *,
@@ -552,32 +565,11 @@ def msda_fused_backward(value, spatial_shapes, level_start_index, reference_poin
     msda_fused_forward.  grad_offsets and grad_logits are bit-deterministic; deterministic=True
     (odise_msda_fused_backward_det_f32) makes grad_value so too.  Box reference points take
     odise_msda_fused_box_backward_f32 / _det_f32."""
-    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
-                                                      offsets, logits, grad_output)
-    box = "box_" if _msda_box(reference_points) else ""
-    fn = f"odise_msda_fused_{box}backward_{'det_' if deterministic else ''}f32"
-    _msda_d32_only(fn, S, M, D, L, P)
-    grad_value = torch.empty_like(value)
-    grad_offs = torch.empty_like(offsets)
-    grad_logits = torch.empty_like(logits)
-    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
-            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
-    if deterministic:
-        rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
-    else:
-        rc = getattr(load(), fn)(*args, _stream())
-    _check(rc, fn)
-    return grad_value, grad_offs, grad_logits
+    return _msda_fused_backward(torch.float32, value, spatial_shapes, level_start_index, reference_points, offsets,
+                                logits, grad_output, deterministic)
 
 
-_MSDA_16BIT = {torch.float16: "f16", torch.bfloat16: "bf16"}
-
-
-def _msda_16bit_suffix(value):
-    if value.dtype not in _MSDA_16BIT:
-        raise OdiseError(f"value: expected float16 or bfloat16, got {value.dtype} (float32 takes msda_fused_forward / "
-                         "msda_fused_backward)")
-    return _MSDA_16BIT[value.dtype]
+_16BIT = (torch.float16, torch.bfloat16)
 
 
 def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
@@ -586,16 +578,7 @@ def msda_fused_forward_16bit(value, spatial_shapes, level_start_index, reference
     of the fp32 result.  D = 32 and L*P <= 32 only.  Box reference points [N, Lq, L, 4] take odise_msda_fused_box_f16 /
     _bf16.  RuntimeError on CPU or non-contiguous tensors, on a float32 value, on mixed dtypes, on shapes that disagree
     and on unsupported shapes."""
-    sfx = _msda_16bit_suffix(value)
-    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
-                                                      offsets, logits, dtype=value.dtype)
-    fn = "odise_msda_fused_" + ("box_" if _msda_box(reference_points) else "") + sfx
-    _msda_d32_only(fn, S, M, D, L, P)
-    out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
-    rc = getattr(load(), fn)(_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits),
-                             _ptr(out), N, S, M, D, L, Lq, P, _stream())
-    _check(rc, fn)
-    return out
+    return _msda_fused_forward(_16BIT, value, spatial_shapes, level_start_index, reference_points, offsets, logits)
 
 
 def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
@@ -606,27 +589,8 @@ def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, referenc
     dtype.  Errors as msda_fused_forward_16bit.  deterministic=True (odise_msda_fused_backward_det_f16 / _bf16) sums
     grad_value in int64 fixed point and the kernels write it in the value's dtype: its bits depend on the inputs only.
     Box reference points take odise_msda_fused_box_backward_* (and _det_*)."""
-    sfx = _msda_16bit_suffix(value)
-    N, S, M, D, L, Lq, P, ss, ls = _msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
-                                                      offsets, logits, grad_output, dtype=value.dtype)
-    box = "box_" if _msda_box(reference_points) else ""
-    fn = f"odise_msda_fused_{box}backward_{'det_' if deterministic else ''}{sfx}"
-    _msda_d32_only(fn, S, M, D, L, P)
-    grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
-    grad_offs = torch.empty_like(offsets)
-    grad_logits = torch.empty_like(logits)
-    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
-            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
-    if deterministic:
-        rc = getattr(load(), fn)(*args, _ptr(_msda_det_workspace(N, S, M, D, value.device)), _stream())
-        _check(rc, fn)
-        return grad_value, grad_offs, grad_logits
-    rc = getattr(load(), fn)(*args, _stream())
-    _check(rc, fn)
-    return grad_value.to(value.dtype), grad_offs, grad_logits
-
-
-_XATTN_SFX = {torch.float32: "f32", torch.float16: "f16", torch.bfloat16: "bf16"}
+    return _msda_fused_backward(_16BIT, value, spatial_shapes, level_start_index, reference_points, offsets, logits,
+                                grad_output, deterministic)
 
 
 def _xattn_shapes(q, k, v, mask, heads, out=None, lse=None, grad_out=None):
@@ -634,17 +598,9 @@ def _xattn_shapes(q, k, v, mask, heads, out=None, lse=None, grad_out=None):
     implementations of odise_b200.masked_attn's ops call it too): q [Q, B, E], k and v [S, B, E], E = heads * 32, CUDA,
     contiguous, one dtype of float32 / float16 / bfloat16; mask None or a contiguous CUDA bool [B*heads, Q, S] or
     [Q, S]; for the backward out and grad_out like q and lse [B*heads, Q] float32.  -> (Q, B, E, S, mask_bh_stride)"""
-    named = [(q, "q"), (k, "k"), (v, "v")] + [(t, n) for t, n in ((out, "out"), (grad_out, "grad_out")) if t is not None]
-    if q.dtype not in _XATTN_SFX:
-        raise OdiseError(f"q: expected float32, float16 or bfloat16, got {q.dtype}")
-    for t, nm in named:
-        if not t.is_cuda:
-            raise OdiseError(f"{nm} must be a CUDA tensor")
-        if not t.is_contiguous():
-            raise OdiseError(f"{nm} tensor has to be contiguous")
-        _req(t, q.dtype, nm)
-        if t.dim() != 3:
-            raise OdiseError(f"{nm}: expected a 3-D tensor, got {tuple(t.shape)}")
+    _tensor(q, "q", _FLOATS)
+    if q.dim() != 3 or k.dim() != 3:
+        raise OdiseError(f"q and k: expected 3-D tensors, got {tuple(q.shape)} and {tuple(k.shape)}")
     Q, B, E = q.shape
     S = k.shape[0]
     if heads <= 0 or E % heads:
@@ -653,29 +609,22 @@ def _xattn_shapes(q, k, v, mask, heads, out=None, lse=None, grad_out=None):
         raise OdiseError(f"masked cross-attention: head dim {E // heads} not supported (32 only)")
     for t, nm, want in ((k, "k", (S, B, E)), (v, "v", (S, B, E)), (out, "out", (Q, B, E)),
                         (grad_out, "grad_out", (Q, B, E))):
-        if t is not None and tuple(t.shape) != want:
-            raise OdiseError(f"{nm}: expected shape {want}, got {tuple(t.shape)}")
+        if t is not None:
+            _tensor(t, nm, q.dtype, want)
     if S <= 0 or Q <= 0 or B <= 0:
         raise OdiseError(f"empty sequence: Q = {Q}, S = {S}, B = {B}")
     if B * heads > 65535 or (S + 63) // 64 > 65535:
         raise OdiseError(f"masked cross-attention: B*heads = {B * heads} or S = {S} too large")
     if lse is not None:
-        if not lse.is_cuda or lse.dtype != torch.float32 or tuple(lse.shape) != (B * heads, Q) or not lse.is_contiguous():
-            raise OdiseError(f"lse: expected a contiguous CUDA float32 tensor of shape {(B * heads, Q)}")
+        _tensor(lse, "lse", torch.float32, (B * heads, Q))
     stride = 0
     if mask is not None:
-        if not mask.is_cuda or mask.dtype != torch.bool or not mask.is_contiguous():
-            raise OdiseError("mask: expected a contiguous CUDA bool tensor (True = blocked)")
-        if tuple(mask.shape) == (B * heads, Q, S):
+        _tensor(mask, "mask", torch.bool)     # True = blocked
+        if mask.shape == (B * heads, Q, S):
             stride = Q * S
-        elif tuple(mask.shape) != (Q, S):
+        elif mask.shape != (Q, S):
             raise OdiseError(f"mask: expected shape {(B * heads, Q, S)} or {(Q, S)}, got {tuple(mask.shape)}")
     return Q, B, E, S, stride
-
-
-def _xattn_workspace(B, H, Q, S, device):
-    """workspace of the masked cross-attention entry points (odise_masked_xattn_workspace_bytes), from torch's allocator"""
-    return torch.empty(int(load().odise_masked_xattn_workspace_bytes(B, H, Q, S)), dtype=torch.uint8, device=device)
 
 
 def masked_xattn_forward(q, k, v, mask, heads):
@@ -686,10 +635,9 @@ def masked_xattn_forward(q, k, v, mask, heads):
     Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads)
     out = torch.empty_like(q)
     lse = torch.empty(B * heads, Q, dtype=torch.float32, device=q.device)
-    ws = _xattn_workspace(B, heads, Q, S, q.device)
-    fn = "odise_masked_xattn_forward_" + _XATTN_SFX[q.dtype]
-    _check(getattr(load(), fn)(_ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out), _ptr(lse), B, heads, 32, Q, S,
-                               _ptr(ws), _stream()), fn)
+    ws = _scratch(load().odise_masked_xattn_workspace_bytes(B, heads, Q, S), q.device)
+    _launch("odise_masked_xattn_forward_" + _SFX[q.dtype], _ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out),
+            _ptr(lse), B, heads, 32, Q, S, _ptr(ws))
     return out, lse
 
 
@@ -699,28 +647,21 @@ def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
     masked_xattn_forward, and for out / lse / grad_out of the wrong shape or dtype."""
     Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads, out=out, lse=lse, grad_out=grad_out)
     gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-    ws = _xattn_workspace(B, heads, Q, S, q.device)
-    fn = "odise_masked_xattn_backward_" + _XATTN_SFX[q.dtype]
-    _check(getattr(load(), fn)(_ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out), _ptr(lse), _ptr(grad_out),
-                               _ptr(gq), _ptr(gk), _ptr(gv), B, heads, 32, Q, S, _ptr(ws), _stream()), fn)
+    ws = _scratch(load().odise_masked_xattn_workspace_bytes(B, heads, Q, S), q.device)
+    _launch("odise_masked_xattn_backward_" + _SFX[q.dtype], _ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out),
+            _ptr(lse), _ptr(grad_out), _ptr(gq), _ptr(gk), _ptr(gv), B, heads, 32, Q, S, _ptr(ws))
     return gq, gk, gv
 
 
 MASK_MAX_IMAGES, MASK_MAX_CANDIDATES, MASK_MAX_POINTS = 256, 53248, 32768    # ODISE_MASK_MAX_* of the header
+_MASK_BYTES = (torch.bool, torch.uint8)
 
 
 def _mask_maps(pred, tgt):
     """Checks shared by the mask-criterion entry points: pred [B, Q, H, W] float32 / float16 / bfloat16 and the target
     masks tgt [sum T, Hg, Wg] bool or uint8, both CUDA and contiguous.  -> (suffix, B, Q, H, W, Hg, Wg)"""
-    if pred.dtype not in _XATTN_SFX:
-        raise OdiseError(f"pred_masks: expected float32, float16 or bfloat16, got {pred.dtype}")
-    if tgt.dtype not in (torch.bool, torch.uint8):
-        raise OdiseError(f"target masks: expected bool or uint8, got {tgt.dtype}")
-    for t, nm in ((pred, "pred_masks"), (tgt, "target masks")):
-        if not t.is_cuda:
-            raise OdiseError(f"{nm} must be a CUDA tensor")
-        if not t.is_contiguous():
-            raise OdiseError(f"{nm} tensor has to be contiguous")
+    _tensor(pred, "pred_masks", _FLOATS)
+    _tensor(tgt, "target masks", _MASK_BYTES)
     if pred.dim() != 4 or tgt.dim() != 3:
         raise OdiseError(f"pred_masks must be [B, Q, H, W] and target masks [T, Hg, Wg], got {tuple(pred.shape)} and "
                          f"{tuple(tgt.shape)}")
@@ -729,13 +670,7 @@ def _mask_maps(pred, tgt):
         raise OdiseError(f"empty maps: pred_masks {tuple(pred.shape)}, target masks {tuple(tgt.shape)}")
     if B > MASK_MAX_IMAGES:
         raise OdiseError(f"mask criterion: at most {MASK_MAX_IMAGES} images, got {B}")
-    return _XATTN_SFX[pred.dtype], B, Q, H, W, tgt.shape[1], tgt.shape[2]
-
-
-def _req_shape(t, dtype, shape, nm):
-    if not t.is_cuda or t.dtype != dtype or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
-        raise OdiseError(f"{nm}: expected a contiguous CUDA {dtype} tensor of shape {tuple(shape)}, got "
-                         f"{t.dtype} {tuple(t.shape)} on {t.device}")
+    return _SFX[pred.dtype], B, Q, H, W, tgt.shape[1], tgt.shape[2]
 
 
 def _u8(t):
@@ -746,18 +681,16 @@ def mask_point_sample(maps, points):
     """detectron2's point_sample on the device, as the mask-criterion kernels sample (odise_mask_point_sample_*):
     maps [N, H, W] float32 / float16 / bfloat16 / bool / uint8, points [N, P, 2] float32 in [0, 1)^2 -> [N, P] float32,
     bit-equal to F.grid_sample(maps[:, None].float(), 2 * points[:, :, None] - 1, align_corners=False)."""
-    sfx = {torch.bool: "u8", torch.uint8: "u8"}.get(maps.dtype) or _XATTN_SFX.get(maps.dtype)
-    if sfx is None:
-        raise OdiseError(f"maps: expected float32, float16, bfloat16, bool or uint8, got {maps.dtype}")
-    if not maps.is_cuda or not maps.is_contiguous() or maps.dim() != 3:
-        raise OdiseError(f"maps: expected a contiguous CUDA tensor [N, H, W], got {tuple(maps.shape)} on {maps.device}")
+    _tensor(maps, "maps", _FLOATS + _MASK_BYTES)
+    if maps.dim() != 3:
+        raise OdiseError(f"maps: expected [N, H, W], got {tuple(maps.shape)}")
     N, H, W = maps.shape
     if points.dim() != 3 or points.shape[0] != N or points.shape[2] != 2:
         raise OdiseError(f"points: expected [{N}, P, 2], got {tuple(points.shape)}")
-    _req_shape(points, torch.float32, tuple(points.shape), "points")
+    _tensor(points, "points", torch.float32)
     out = torch.empty(N, points.shape[1], dtype=torch.float32, device=maps.device)
-    fn = "odise_mask_point_sample_" + sfx
-    _check(getattr(load(), fn)(_ptr(_u8(maps)), _ptr(points), _ptr(out), N, H, W, points.shape[1], _stream()), fn)
+    _launch("odise_mask_point_sample_" + _SFX[maps.dtype], _ptr(_u8(maps)), _ptr(points), _ptr(out), N, H, W,
+            points.shape[1])
     return out
 
 
@@ -777,18 +710,16 @@ def mask_cost(pred, prob, labels, tgt, points, counts, w_class, w_mask, w_dice, 
     if points.dim() != 3 or points.shape[0] != B or points.shape[2] != 2 or points.shape[1] <= 0:
         raise OdiseError(f"points: expected [{B}, P, 2] with P > 0, got {tuple(points.shape)}")
     P = points.shape[1]
-    _req_shape(prob, torch.float32, (B, Q, K1), "prob")
-    _req_shape(labels, torch.int64, (tgt.shape[0],), "labels")
-    _req_shape(points, torch.float32, (B, P, 2), "points")
+    _tensor(prob, "prob", torch.float32)
+    _tensor(labels, "labels", torch.int64, (tgt.shape[0],))
+    _tensor(points, "points", torch.float32)
     Tmax = max(counts, default=0)
     if out is None:
         out = torch.empty(B, Q, Tmax, dtype=torch.float32, device=pred.device)
-    _req_shape(out, torch.float32, (B, Q, Tmax), "out")
+    _tensor(out, "out", torch.float32, (B, Q, Tmax))
     cnt = (ctypes.c_int * B)(*counts)
-    fn = "odise_mask_cost_" + sfx
-    _check(getattr(load(), fn)(_ptr(pred), _ptr(prob), _ptr(labels), _ptr(_u8(tgt)), _ptr(points), cnt, _ptr(out),
-                               B, Q, H, W, K1, Hg, Wg, Tmax, P, float(w_class), float(w_mask), float(w_dice),
-                               _stream()), fn)
+    _launch("odise_mask_cost_" + sfx, _ptr(pred), _ptr(prob), _ptr(labels), _ptr(_u8(tgt)), _ptr(points), cnt,
+            _ptr(out), B, Q, H, W, K1, Hg, Wg, Tmax, P, float(w_class), float(w_mask), float(w_dice))
     return out
 
 
@@ -798,7 +729,7 @@ def _mask_loss_shapes(pred, tgt, pairs, num_points):
     sfx, B, Q, H, W, Hg, Wg = _mask_maps(pred, tgt)
     if pairs.dim() != 2 or pairs.shape[1] != 3:
         raise OdiseError(f"pairs must be [N, 3], got {tuple(pairs.shape)}")
-    _req_shape(pairs, torch.int64, tuple(pairs.shape), "pairs")
+    _tensor(pairs, "pairs", torch.int64)
     if not 0 < num_points <= MASK_MAX_POINTS:
         raise OdiseError(f"mask loss: num_points = {num_points} not supported (1 .. {MASK_MAX_POINTS})")
     return sfx, B, Q, H, W, Hg, Wg, pairs.shape[0]
@@ -817,14 +748,13 @@ def mask_loss_forward(pred, tgt, pairs, cand, rnd, num_masks, num_points, k):
     if not (S <= MASK_MAX_CANDIDATES and 0 <= k <= min(num_points, S)):
         raise OdiseError(f"mask loss: {S} candidates, k = {k} not supported (candidates <= {MASK_MAX_CANDIDATES}, "
                          f"k <= min(num_points, candidates))")
-    _req_shape(cand, torch.float32, (N, S, 2), "cand")
-    _req_shape(rnd, torch.float32, (N, num_points - k, 2), "rnd")
-    ws = torch.empty(max(int(load().odise_mask_loss_workspace_bytes(N, num_points)), 16), dtype=torch.uint8,
-                     device=pred.device)
+    _tensor(cand, "cand", torch.float32, (N, S, 2))
+    _tensor(rnd, "rnd", torch.float32, (N, num_points - k, 2))
+    # at least 16 bytes: the buffer is also the state mask_loss_backward takes, never empty
+    ws = _scratch(max(load().odise_mask_loss_workspace_bytes(N, num_points), 16), pred.device)
     losses = torch.empty(2, dtype=torch.float32, device=pred.device)
-    fn = "odise_mask_loss_forward_" + sfx
-    _check(getattr(load(), fn)(_ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(cand), _ptr(rnd), _ptr(ws), _ptr(losses),
-                               B, Q, H, W, Hg, Wg, N, num_points, S, k, float(num_masks), _stream()), fn)
+    _launch("odise_mask_loss_forward_" + sfx, _ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(cand), _ptr(rnd), _ptr(ws),
+            _ptr(losses), B, Q, H, W, Hg, Wg, N, num_points, S, k, float(num_masks))
     return losses, ws
 
 
@@ -833,14 +763,13 @@ def mask_loss_backward(pred, tgt, pairs, pair_of, state, grad_losses, num_masks,
     device -> grad_pred shaped and typed like pred, zero on the queries pair_of [B*Q] int64 maps to -1.
     Bit-reproducible (int64 fixed-point sums)."""
     sfx, B, Q, H, W, Hg, Wg, N = _mask_loss_shapes(pred, tgt, pairs, num_points)
-    _req_shape(pair_of, torch.int64, (B * Q,), "pair_of")
-    _req_shape(grad_losses, torch.float32, (2,), "grad_losses")
+    _tensor(pair_of, "pair_of", torch.int64, (B * Q,))
+    _tensor(grad_losses, "grad_losses", torch.float32, (2,))
     if not state.is_cuda or state.dtype != torch.uint8 or state.numel() < N * (16 + 8 * num_points):
         raise OdiseError("state: expected the workspace mask_loss_forward returned")
     grad = torch.empty_like(pred)
-    fn = "odise_mask_loss_backward_" + sfx
-    _check(getattr(load(), fn)(_ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(pair_of), _ptr(state), _ptr(grad_losses),
-                               _ptr(grad), B, Q, H, W, Hg, Wg, N, num_points, float(num_masks), _stream()), fn)
+    _launch("odise_mask_loss_backward_" + sfx, _ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(pair_of), _ptr(state),
+            _ptr(grad_losses), _ptr(grad), B, Q, H, W, Hg, Wg, N, num_points, float(num_masks))
     return grad
 
 
@@ -852,8 +781,7 @@ def _mask_head_shapes(embed, features, outputs_mask=None, weights=None, grad_mas
     odise_b200.decoder's ops call it too): embed [B, Q, 256] and features [B, 256, H, W] contiguous CUDA tensors of one
     dtype of float32 / float16 / bfloat16, Q <= 256, H * W < 2^24; for the backward outputs_mask and grad_mask
     [B, Q, H, W] and grad_pooled [B, Q, 256] of that dtype and weights [B, Q] float32.  -> (suffix, B, Q, H, W)"""
-    if embed.dtype not in _XATTN_SFX:
-        raise OdiseError(f"mask_embed: expected float32, float16 or bfloat16, got {embed.dtype}")
+    _tensor(embed, "mask_embed", _FLOATS)
     if embed.dim() != 3 or features.dim() != 4:
         raise OdiseError(f"mask_embed must be [B, Q, C] and mask_features [B, C, H, W], got {tuple(embed.shape)} and "
                          f"{tuple(features.shape)}")
@@ -863,21 +791,13 @@ def _mask_head_shapes(embed, features, outputs_mask=None, weights=None, grad_mas
         raise OdiseError(f"mask head: C = {C}, Q = {Q} not supported (C = {MASK_HEAD_C}, Q <= {MASK_HEAD_MAX_Q})")
     if min(B, H, W) <= 0 or H * W >= 2 ** 24 or B > 65535:
         raise OdiseError(f"mask head: B = {B}, H x W = {H} x {W} not supported (B <= 65535, 0 < H*W < 2^24)")
-    want = {"mask_features": (B, C, H, W), "outputs_mask": (B, Q, H, W), "grad_mask": (B, Q, H, W),
-            "grad_pooled": (B, Q, C)}
-    for t, nm in ((embed, "mask_embed"), (features, "mask_features"), (outputs_mask, "outputs_mask"),
-                  (grad_mask, "grad_mask"), (grad_pooled, "grad_pooled")):
+    for t, nm, want in ((features, "mask_features", (B, C, H, W)), (outputs_mask, "outputs_mask", (B, Q, H, W)),
+                        (grad_mask, "grad_mask", (B, Q, H, W)), (grad_pooled, "grad_pooled", (B, Q, C))):
         if t is not None:
-            _req_shape(t, embed.dtype, want.get(nm, tuple(embed.shape)), nm)
+            _tensor(t, nm, embed.dtype, want)
     if weights is not None:
-        _req_shape(weights, torch.float32, (B, Q), "weights")
-    return _XATTN_SFX[embed.dtype], B, Q, H, W
-
-
-def _mask_head_workspace(B, Q, H, W, device):
-    """workspace of the mask-head entry points (odise_mask_head_workspace_bytes), from torch's allocator"""
-    return torch.empty(int(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W)), dtype=torch.uint8,
-                       device=device)
+        _tensor(weights, "weights", torch.float32, (B, Q))
+    return _SFX[embed.dtype], B, Q, H, W
 
 
 def mask_head_forward(embed, features, threshold=0.5):
@@ -889,26 +809,23 @@ def mask_head_forward(embed, features, threshold=0.5):
     om = torch.empty(B, Q, H, W, dtype=embed.dtype, device=embed.device)
     pooled = torch.empty_like(embed)
     weights = torch.empty(B, Q, dtype=torch.float32, device=embed.device)
-    ws = _mask_head_workspace(B, Q, H, W, embed.device)
-    fn = "odise_mask_head_forward_" + sfx
-    _check(getattr(load(), fn)(_ptr(embed), _ptr(features), _ptr(om), _ptr(pooled), _ptr(weights), B, Q, MASK_HEAD_C,
-                               H, W, float(threshold), _ptr(ws), _stream()), fn)
+    ws = _scratch(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W), embed.device)
+    _launch("odise_mask_head_forward_" + sfx, _ptr(embed), _ptr(features), _ptr(om), _ptr(pooled), _ptr(weights), B, Q,
+            MASK_HEAD_C, H, W, float(threshold), _ptr(ws))
     return om, pooled, weights
 
 
 def _mask_head_attn_shapes(outputs_mask, size, heads):
     """Checks of mask_head_attn_mask (shared with its fake): -> (suffix, B, Q, H, W, h, w)"""
-    if outputs_mask.dtype not in _XATTN_SFX:
-        raise OdiseError(f"outputs_mask: expected float32, float16 or bfloat16, got {outputs_mask.dtype}")
+    _tensor(outputs_mask, "outputs_mask", _FLOATS)
     if outputs_mask.dim() != 4:
         raise OdiseError(f"outputs_mask must be [B, Q, H, W], got {tuple(outputs_mask.shape)}")
-    _req_shape(outputs_mask, outputs_mask.dtype, tuple(outputs_mask.shape), "outputs_mask")
     B, Q, H, W = outputs_mask.shape
     h, w = (int(s) for s in size)
     if min(B, Q, H, W, h, w, heads) <= 0 or B * Q >= 2 ** 31 or h * w >= 2 ** 31:
         raise OdiseError(f"attention mask: outputs_mask {tuple(outputs_mask.shape)}, size {(h, w)}, heads {heads} not "
                          "supported")
-    return _XATTN_SFX[outputs_mask.dtype], B, Q, H, W, h, w
+    return _SFX[outputs_mask.dtype], B, Q, H, W, h, w
 
 
 def mask_head_attn_mask(outputs_mask, size, heads):
@@ -917,8 +834,7 @@ def mask_head_attn_mask(outputs_mask, size, heads):
     dtype, with every all-blocked row written all False (odise.py:683)."""
     sfx, B, Q, H, W, h, w = _mask_head_attn_shapes(outputs_mask, size, heads)
     out = torch.empty(B * heads, Q, h * w, dtype=torch.bool, device=outputs_mask.device)
-    fn = "odise_mask_head_attn_mask_" + sfx
-    _check(getattr(load(), fn)(_ptr(outputs_mask), _ptr(out), B, Q, H, W, h, w, heads, _stream()), fn)
+    _launch("odise_mask_head_attn_mask_" + sfx, _ptr(outputs_mask), _ptr(out), B, Q, H, W, h, w, heads)
     return out
 
 
@@ -929,11 +845,9 @@ def mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_p
     shape or dtype."""
     sfx, B, Q, H, W = _mask_head_shapes(embed, features, outputs_mask, weights, grad_mask, grad_pooled)
     ge, gx = torch.empty_like(embed), torch.empty_like(features)
-    ws = _mask_head_workspace(B, Q, H, W, embed.device)
-    fn = "odise_mask_head_backward_" + sfx
-    _check(getattr(load(), fn)(_ptr(embed), _ptr(features), _ptr(outputs_mask), _ptr(weights), _ptr(grad_mask),
-                               _ptr(grad_pooled), _ptr(ge), _ptr(gx), B, Q, MASK_HEAD_C, H, W, float(threshold),
-                               _ptr(ws), _stream()), fn)
+    ws = _scratch(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W), embed.device)
+    _launch("odise_mask_head_backward_" + sfx, _ptr(embed), _ptr(features), _ptr(outputs_mask), _ptr(weights),
+            _ptr(grad_mask), _ptr(grad_pooled), _ptr(ge), _ptr(gx), B, Q, MASK_HEAD_C, H, W, float(threshold), _ptr(ws))
     return ge, gx
 
 
@@ -948,8 +862,7 @@ def _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_star
     null_embed [1, C] of mask_embed's dtype or (16-bit mask_embed only) both float32, logit_scale a float32 scalar,
     group_start int32 [K + 1], all contiguous CUDA tensors; for the backward winners uint8 and grad_logits of
     mask_embed's dtype [B, Q, K + 1], norms float32 [B*Q + Kp + 1].  -> (suffix, bank_f32, B, Q, C, K, Kp)"""
-    if mask_embed.dtype not in _XATTN_SFX:
-        raise OdiseError(f"mask_embed: expected float32, float16 or bfloat16, got {mask_embed.dtype}")
+    _tensor(mask_embed, "mask_embed", _FLOATS)
     if mask_embed.dim() != 3 or text_embed.dim() != 2 or group_start.dim() != 1:
         raise OdiseError(f"mask_embed must be [B, Q, C], text_embed [Kp, C] and group_start [K + 1], got "
                          f"{tuple(mask_embed.shape)}, {tuple(text_embed.shape)} and {tuple(group_start.shape)}")
@@ -959,21 +872,17 @@ def _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_star
             or Kp > CATEGORY_MAX_PROMPTS or B * Q * max(K + 1, C) >= 2 ** 31:
         raise OdiseError(f"category scoring: B = {B}, Q = {Q}, C = {C}, K = {K}, Kp = {Kp} not supported (C a multiple "
                          f"of {CATEGORY_C_MULTIPLE} up to {CATEGORY_MAX_C}, 1 <= K <= Kp <= {CATEGORY_MAX_PROMPTS})")
-    bank = text_embed.dtype
-    if bank != mask_embed.dtype and not (bank == torch.float32 and mask_embed.dtype != torch.float32):
-        raise OdiseError(f"text_embed: expected {mask_embed.dtype} or (16-bit mask_embed) float32, got {bank}")
-    _req_shape(mask_embed, mask_embed.dtype, (B, Q, C), "mask_embed")
-    _req_shape(text_embed, bank, (Kp, C), "text_embed")
-    _req_shape(null_embed, bank, (1, C), "null_embed")
-    _req_shape(logit_scale, torch.float32, (), "logit_scale")
-    _req_shape(group_start, torch.int32, (K + 1,), "group_start")
+    _tensor(text_embed, "text_embed", (mask_embed.dtype, torch.float32), (Kp, C))    # float32 = a float32 bank
+    _tensor(null_embed, "null_embed", text_embed.dtype, (1, C))
+    _tensor(logit_scale, "logit_scale", torch.float32, ())
+    _tensor(group_start, "group_start", torch.int32)
     if winners is not None:
-        _req_shape(winners, torch.uint8, (B, Q, K + 1), "winners")
+        _tensor(winners, "winners", torch.uint8, (B, Q, K + 1))
     if norms is not None:
-        _req_shape(norms, torch.float32, (B * Q + Kp + 1,), "norms")
+        _tensor(norms, "norms", torch.float32, (B * Q + Kp + 1,))
     if grad_logits is not None:
-        _req_shape(grad_logits, mask_embed.dtype, (B, Q, K + 1), "grad_logits")
-    return _XATTN_SFX[mask_embed.dtype], int(bank != mask_embed.dtype), B, Q, C, K, Kp
+        _tensor(grad_logits, "grad_logits", mask_embed.dtype, (B, Q, K + 1))
+    return _SFX[mask_embed.dtype], int(text_embed.dtype != mask_embed.dtype), B, Q, C, K, Kp
 
 
 def category_group_start(sizes):
@@ -998,10 +907,8 @@ def category_logits_forward(mask_embed, text_embed, null_embed, logit_scale, gro
     out = torch.empty(B, Q, K + 1, dtype=mask_embed.dtype, device=dev)
     win = torch.empty(B, Q, K + 1, dtype=torch.uint8, device=dev)
     norms = torch.empty(B * Q + Kp + 1, dtype=torch.float32, device=dev)
-    fn = "odise_category_logits_forward_" + sfx
-    _check(getattr(load(), fn)(_ptr(mask_embed), _ptr(text_embed), _ptr(null_embed), _ptr(logit_scale),
-                               _ptr(group_start), _ptr(out), _ptr(win), _ptr(norms), B * Q, C, K, Kp, bank_f32,
-                               _stream()), fn)
+    _launch("odise_category_logits_forward_" + sfx, _ptr(mask_embed), _ptr(text_embed), _ptr(null_embed),
+            _ptr(logit_scale), _ptr(group_start), _ptr(out), _ptr(win), _ptr(norms), B * Q, C, K, Kp, bank_f32)
     return out, win, norms
 
 
@@ -1014,12 +921,10 @@ def category_logits_backward(mask_embed, text_embed, null_embed, logit_scale, gr
                                                      winners, norms, grad_logits)
     gm, gt, gn = torch.empty_like(mask_embed), torch.empty_like(text_embed), torch.empty_like(null_embed)
     gs = torch.empty((), dtype=torch.float32, device=mask_embed.device)
-    ws = torch.empty(int(load().odise_category_logits_workspace_bytes(B * Q, C, K, Kp)), dtype=torch.uint8,
-                     device=mask_embed.device)
-    fn = "odise_category_logits_backward_" + sfx
-    _check(getattr(load(), fn)(_ptr(mask_embed), _ptr(text_embed), _ptr(null_embed), _ptr(logit_scale),
-                               _ptr(group_start), _ptr(winners), _ptr(norms), _ptr(grad_logits), _ptr(gm), _ptr(gt),
-                               _ptr(gn), _ptr(gs), B * Q, C, K, Kp, bank_f32, _ptr(ws), _stream()), fn)
+    ws = _scratch(load().odise_category_logits_workspace_bytes(B * Q, C, K, Kp), mask_embed.device)
+    _launch("odise_category_logits_backward_" + sfx, _ptr(mask_embed), _ptr(text_embed), _ptr(null_embed),
+            _ptr(logit_scale), _ptr(group_start), _ptr(winners), _ptr(norms), _ptr(grad_logits), _ptr(gm), _ptr(gt),
+            _ptr(gn), _ptr(gs), B * Q, C, K, Kp, bank_f32, _ptr(ws))
     return gm, gt, gn, gs
 
 
@@ -1030,7 +935,7 @@ def _fpn_nchw(t, name):
     """-> (N, C, H, W) of an NCHW-contiguous CUDA float32 operand of the FPN upsample-add kernels, checked"""
     if t.dim() != 4:
         raise OdiseError(f"{name} must be [N, C, H, W], got {tuple(t.shape)}")
-    _req_shape(t, torch.float32, tuple(t.shape), name)
+    _tensor(t, name, torch.float32)
     return tuple(t.shape)
 
 
@@ -1049,10 +954,7 @@ def _fpn_shapes(z, cur, size):
     -> (N, C, h, w, H, W, batch stride of z)"""
     h, w = (int(s) for s in size)
     N, C, H, W = _fpn_nchw(cur, "cur")
-    if not z.is_cuda or z.dtype != torch.float32:
-        raise OdiseError(f"z: expected a CUDA float32 tensor, got {z.dtype} on {z.device}")
-    if tuple(z.shape) != (N, h * w, C):
-        raise OdiseError(f"z: expected shape {(N, h * w, C)} (cur {(N, C, H, W)}, level {h}x{w}), got {tuple(z.shape)}")
+    _tensor(z, "z", torch.float32, (N, h * w, C), contiguous=False)
     _fpn_limits(N, C, h, w, H, W)
     bs = z.stride(0) if N > 1 else h * w * C
     if z.stride(2) != 1 or (h * w > 1 and z.stride(1) != C) or bs < h * w * C:
@@ -1067,8 +969,7 @@ def fpn_upsample_add(z, cur, size):
     take."""
     N, C, h, w, H, W, bs = _fpn_shapes(z, cur, size)
     y = torch.empty_like(cur)
-    fn = "odise_fpn_upsample_add_f32"
-    _check(getattr(load(), fn)(_ptr(z), bs, _ptr(cur), _ptr(y), N, C, h, w, H, W, _stream()), fn)
+    _launch("odise_fpn_upsample_add_f32", _ptr(z), bs, _ptr(cur), _ptr(y), N, C, h, w, H, W)
     return y
 
 
@@ -1086,8 +987,7 @@ def fpn_upsample_add_backward(grad_y, size):
     without atomics (bit-reproducible).  The gradient of cur is grad_y itself."""
     N, C, h, w, H, W = _fpn_backward_shapes(grad_y, size)
     gz = torch.empty(N, h * w, C, dtype=torch.float32, device=grad_y.device)
-    fn = "odise_fpn_upsample_add_backward_f32"
-    _check(getattr(load(), fn)(_ptr(grad_y), _ptr(gz), h * w * C, N, C, h, w, H, W, _stream()), fn)
+    _launch("odise_fpn_upsample_add_backward_f32", _ptr(grad_y), _ptr(gz), h * w * C, N, C, h, w, H, W)
     return gz
 
 

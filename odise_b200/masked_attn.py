@@ -20,13 +20,12 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from . import lib
-from . import msda as _msda  # noqa: F401  (holds the "DEF" library of the odise_b200 namespace; defined first)
 
 _DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 
-# The kernels as custom ops in the odise_b200 namespace (odise_b200.msda holds the namespace's "DEF" library, so this
-# module adds to it as a fragment).  As for the MSDA ops: the implementation is registered for every device so that a
-# CPU tensor reaches lib's own check, and the fakes refuse what lib refuses for reasons visible without data.
+# The kernels as custom ops in the odise_b200 namespace.  As for the MSDA ops: the implementation is registered for every
+# device so that a CPU tensor reaches lib's own check, and the fakes refuse what lib refuses for reasons visible without
+# data.
 _OPS = torch.library.Library("odise_b200", "FRAGMENT")
 _OPS.define("masked_xattn_forward(Tensor q, Tensor k, Tensor v, Tensor? mask, int heads) -> (Tensor, Tensor)")
 _OPS.define("masked_xattn_backward(Tensor q, Tensor k, Tensor v, Tensor? mask, Tensor out, Tensor lse, "

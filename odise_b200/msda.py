@@ -35,7 +35,7 @@ from . import lib
 # torch.library.Library rather than torch.library.custom_op: its eager call goes straight to the dispatcher, without
 # custom_op's Python wrapper (DESIGN.md §3, "Under torch.compile").  There is no autograd formula on the ops: the Functions below are the
 # one autograd definition, and Dynamo traces them with the ops inside.
-_OPS = torch.library.Library("odise_b200", "DEF")
+_OPS = torch.library.Library("odise_b200", "FRAGMENT")
 _OPS.define("msda_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
             "Tensor attn_weight, int im2col_step) -> Tensor")
 _OPS.define("msda_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
@@ -94,31 +94,18 @@ def _msda_backward_fake(value, spatial_shapes, level_start_index, sampling_loc, 
     return torch.empty_like(value), torch.empty_like(sampling_loc), torch.empty_like(attn_weight)
 
 
-def _msda_fused_fake_shapes(op, value, spatial_shapes, level_start_index, reference_points, offsets, logits,
-                            grad_output=None):
-    """lib's checks of the fused op `op` (forward when grad_output is None) for value's dtype and reference-point width
-    -> (N, Lq, M, D)"""
-    low = value.dtype in _LOW
-    N, S, M, D, L, Lq, P, _, _ = lib._msda_fused_shapes(value, spatial_shapes, level_start_index, reference_points,
-                                                        offsets, logits, grad_output,
-                                                        dtype=value.dtype if low else torch.float32)
-    if low or grad_output is not None or lib._msda_box(reference_points):
-        lib._msda_d32_only(op, S, M, D, L, P)
-    return N, Lq, M, D
-
-
 @torch.library.register_fake("odise_b200::msda_fused_forward", lib=_OPS)
 def _msda_fused_forward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
-    N, Lq, M, D = _msda_fused_fake_shapes("odise_b200::msda_fused_forward", value, spatial_shapes, level_start_index,
-                                          reference_points, offsets, logits)
+    _, N, S, M, D, L, Lq, P = lib._msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets,
+                                                   logits)
     return value.new_empty(N, Lq, M * D)
 
 
 @torch.library.register_fake("odise_b200::msda_fused_backward", lib=_OPS)
 def _msda_fused_backward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
                               deterministic):
-    _msda_fused_fake_shapes("odise_b200::msda_fused_backward", value, spatial_shapes, level_start_index,
-                            reference_points, offsets, logits, grad_output)
+    lib._msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
+                         deterministic)
     return torch.empty_like(value), torch.empty_like(offsets), torch.empty_like(logits)
 
 
