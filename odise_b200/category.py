@@ -30,39 +30,13 @@ from torch.autograd.function import once_differentiable
 
 from . import lib
 
-_OPS = torch.library.Library("odise_b200", "FRAGMENT")
-_OPS.define("category_logits(Tensor mask_embed, Tensor text_embed, Tensor null_embed, Tensor logit_scale, "
-            "Tensor group_start) -> (Tensor, Tensor, Tensor)")
-_OPS.define("category_logits_backward(Tensor mask_embed, Tensor text_embed, Tensor null_embed, Tensor logit_scale, "
-            "Tensor group_start, Tensor winners, Tensor norms, Tensor grad_logits) -> (Tensor, Tensor, Tensor, Tensor)")
-
-
-# lib's functions are looked up at call time, so that a test that patches them sees every call
-def _forward(mask_embed, text_embed, null_embed, logit_scale, group_start):
-    return lib.category_logits_forward(mask_embed, text_embed, null_embed, logit_scale, group_start)
-
-
-def _backward(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits):
-    return lib.category_logits_backward(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms,
-                                        grad_logits)
-
-
-_OPS.impl("category_logits", _forward, "CompositeExplicitAutograd")
-_OPS.impl("category_logits_backward", _backward, "CompositeExplicitAutograd")
-
-
-@torch.library.register_fake("odise_b200::category_logits", lib=_OPS)
-def _forward_fake(mask_embed, text_embed, null_embed, logit_scale, group_start):
-    _, _, B, Q, C, K, Kp = lib._category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start)
-    return (mask_embed.new_empty(B, Q, K + 1), mask_embed.new_empty(B, Q, K + 1, dtype=torch.uint8),
-            mask_embed.new_empty(B * Q + Kp + 1, dtype=torch.float32))
-
-
-@torch.library.register_fake("odise_b200::category_logits_backward", lib=_OPS)
-def _backward_fake(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits):
-    lib._category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start, winners, norms, grad_logits)
-    return (torch.empty_like(mask_embed), torch.empty_like(text_embed), torch.empty_like(null_embed),
-            torch.empty_like(logit_scale))
+# The kernels as torch custom ops (lib.custom_op).  lib's functions are looked up at call time, so that a test that
+# patches them sees every call.
+lib.custom_op("category_logits(Tensor mask_embed, Tensor text_embed, Tensor null_embed, Tensor logit_scale, "
+              "Tensor group_start) -> (Tensor, Tensor, Tensor)", lambda *args: lib.category_logits_forward(*args))
+lib.custom_op("category_logits_backward(Tensor mask_embed, Tensor text_embed, Tensor null_embed, Tensor logit_scale, "
+              "Tensor group_start, Tensor winners, Tensor norms, Tensor grad_logits) -> (Tensor, Tensor, Tensor, Tensor)",
+              lambda *args: lib.category_logits_backward(*args))
 
 
 class CategoryLogitsFunction(Function):

@@ -33,47 +33,14 @@ from torch.autograd.function import once_differentiable
 from . import lib
 from .masked_attn import CrossAttentionLayer, _activation
 
-_OPS = torch.library.Library("odise_b200", "FRAGMENT")
-_OPS.define("mask_head_forward(Tensor embed, Tensor features, float threshold) -> (Tensor, Tensor, Tensor)")
-_OPS.define("mask_head_backward(Tensor embed, Tensor features, Tensor outputs_mask, Tensor weights, Tensor grad_mask, "
-            "Tensor grad_pooled, float threshold) -> (Tensor, Tensor)")
-_OPS.define("mask_head_attn_mask(Tensor outputs_mask, int h, int w, int heads) -> Tensor")
-
-
-# lib's functions are looked up at call time, so that a test that patches them sees every call
-def _forward(embed, features, threshold):
-    return lib.mask_head_forward(embed, features, threshold)
-
-
-def _backward(embed, features, outputs_mask, weights, grad_mask, grad_pooled, threshold):
-    return lib.mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_pooled, threshold)
-
-
-def _attn_mask(outputs_mask, h, w, heads):
-    return lib.mask_head_attn_mask(outputs_mask, (h, w), heads)
-
-
-_OPS.impl("mask_head_forward", _forward, "CompositeExplicitAutograd")
-_OPS.impl("mask_head_backward", _backward, "CompositeExplicitAutograd")
-_OPS.impl("mask_head_attn_mask", _attn_mask, "CompositeExplicitAutograd")
-
-
-@torch.library.register_fake("odise_b200::mask_head_forward", lib=_OPS)
-def _forward_fake(embed, features, threshold):
-    _, B, Q, H, W = lib._mask_head_shapes(embed, features)
-    return embed.new_empty(B, Q, H, W), torch.empty_like(embed), embed.new_empty(B, Q, dtype=torch.float32)
-
-
-@torch.library.register_fake("odise_b200::mask_head_backward", lib=_OPS)
-def _backward_fake(embed, features, outputs_mask, weights, grad_mask, grad_pooled, threshold):
-    lib._mask_head_shapes(embed, features, outputs_mask, weights, grad_mask, grad_pooled)
-    return torch.empty_like(embed), torch.empty_like(features)
-
-
-@torch.library.register_fake("odise_b200::mask_head_attn_mask", lib=_OPS)
-def _attn_mask_fake(outputs_mask, h, w, heads):
-    _, B, Q, H, W, h, w = lib._mask_head_attn_shapes(outputs_mask, (h, w), heads)
-    return outputs_mask.new_empty(B * heads, Q, h * w, dtype=torch.bool)
+# The kernels as torch custom ops (lib.custom_op).  lib's functions are looked up at call time, so that a test that
+# patches them sees every call.
+lib.custom_op("mask_head_forward(Tensor embed, Tensor features, float threshold) -> (Tensor, Tensor, Tensor)",
+              lambda *args: lib.mask_head_forward(*args))
+lib.custom_op("mask_head_backward(Tensor embed, Tensor features, Tensor outputs_mask, Tensor weights, Tensor grad_mask, "
+              "Tensor grad_pooled, float threshold) -> (Tensor, Tensor)", lambda *args: lib.mask_head_backward(*args))
+lib.custom_op("mask_head_attn_mask(Tensor outputs_mask, int h, int w, int heads) -> Tensor",
+              lambda outputs_mask, h, w, heads: lib.mask_head_attn_mask(outputs_mask, (h, w), heads))
 
 
 class MaskHeadFunction(Function):

@@ -3,6 +3,7 @@
 PyTorch is used for device memory and streams only; every op here launches hand-written sm_90a kernels through
 the C ABI.  There is NO fallback: if the library is missing or a call fails, an exception is raised.
 """
+import contextvars
 import ctypes
 import os
 import re
@@ -108,9 +109,50 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _launch(name, *args):
-    """Run entry point `name` with args on the current stream; OdiseError if it returns an error code."""
-    _check(getattr(load(), name)(*args, _stream()), name)
+# set while a custom op's fake implementation runs (custom_op): _launch then returns before loading the library
+_NO_LAUNCH = contextvars.ContextVar("odise_b200_no_launch", default=False)
+_Tensor = torch.Tensor
+
+
+def _launch(name, *args, workspace=None):
+    """Run entry point `name` on the current stream; OdiseError if it returns an error code.  Tensor arguments are
+    passed as their addresses; ints, floats, None and ctypes arrays as they are.  workspace, if given, maps the loaded
+    library to a byte count: a _scratch buffer of that size on the first argument's device goes last."""
+    if _NO_LAUNCH.get():
+        return
+    dll = load()
+    if workspace is not None:
+        args += (_scratch(workspace(dll), args[0].device),)
+    # None and ints are tested first: isinstance against torch.Tensor (a class with a metaclass) is slow for them
+    _check(getattr(dll, name)(*[a if a is None or type(a) is int else a.data_ptr() if isinstance(a, _Tensor) else a
+                                for a in args], _stream()), name)
+
+
+# The training drop-ins' kernels as torch custom ops in namespace odise_b200, the one place where a traced graph
+# (torch.compile, torch.export) meets the ctypes calls, which Dynamo cannot trace.  torch.library.Library rather than
+# torch.library.custom_op: its eager call goes straight to the dispatcher, without custom_op's Python wrapper (DESIGN.md
+# §3, "Under torch.compile").
+_OPS = torch.library.Library("odise_b200", "FRAGMENT")
+
+
+def custom_op(schema, impl):
+    """Define torch.ops.odise_b200.<name> by its schema and run it with impl, a call of a wrapper of this module, on
+    every device, so that a CPU tensor reaches the wrapper's own check.  The fake implementation is the same impl with
+    launching switched off: the wrapper's checks read no data and need no library, so the fake refuses what the real
+    call refuses for reasons visible without data, and allocates exactly the results the real call returns.  The ops
+    have no autograd formula: each drop-in's autograd.Function is the one autograd definition, and Dynamo traces it with
+    the ops inside."""
+    name = schema.split("(")[0]
+    _OPS.define(schema)
+    _OPS.impl(name, impl, "CompositeExplicitAutograd")
+
+    def fake(*args, **kwargs):
+        token = _NO_LAUNCH.set(True)
+        try:
+            return impl(*args, **kwargs)
+        finally:
+            _NO_LAUNCH.reset(token)
+    torch.library.register_fake(f"odise_b200::{name}", fake, lib=_OPS)
 
 
 # the entry-point suffix of each storage dtype (bool masks are read as bytes); each wrapper states which dtypes it takes
@@ -121,8 +163,7 @@ _FLOATS = (torch.float32, torch.float16, torch.bfloat16)     # the storage types
 
 def _tensor(t, name, dtypes, shape=None, contiguous=True):
     """Raise OdiseError unless t is a CUDA tensor of `dtypes` (one dtype or a tuple), contiguous (unless
-    contiguous=False: strided operands) and, if given, of `shape`.  Reads no data, so the fake implementations of the
-    custom ops check with it too."""
+    contiguous=False: strided operands) and, if given, of `shape`.  Reads no data and needs no library."""
     dtypes = dtypes if isinstance(dtypes, tuple) else (dtypes,)
     if not t.is_cuda:
         raise OdiseError(f"{name} must be a CUDA tensor")
@@ -416,8 +457,7 @@ def _msda_forward(dtypes, value, spatial_shapes, level_start_index, sampling_loc
     _, Lq, _, L, P, _ = sampling_locations.shape
     ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
     out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
-    _launch("odise_msda_forward_" + sfx, _ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_locations),
-            _ptr(attention_weights), _ptr(out), N, S, M, D, L, Lq, P)
+    _launch("odise_msda_forward_" + sfx, value, ss, ls, sampling_locations, attention_weights, out, N, S, M, D, L, Lq, P)
     return out
 
 
@@ -434,16 +474,6 @@ def msda_forward_f64(value, spatial_shapes, level_start_index, sampling_location
                          attention_weights, im2col_step)
 
 
-def _msda_backward_shapes(value, sampling_loc, grad_output):
-    """(N, S, M, D, L, Lq, P) of msda_backward's layouts (value [N, S, M, D], sampling_loc [N, Lq, M, L, P, 2]); raises
-    unless grad_output has N * Lq * M * D elements."""
-    N, S, M, D = value.shape
-    _, Lq, _, L, P, _ = sampling_loc.shape
-    if grad_output.numel() != N * Lq * M * D:
-        raise OdiseError(f"grad_output: expected {N * Lq * M * D} elements, got {grad_output.numel()}")
-    return N, S, M, D, L, Lq, P
-
-
 def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step=128,
                   *, deterministic=False):
     """Drop-in for MSDA.ms_deform_attn_backward (reference ops/src/vision.cpp:20): same arguments, returns
@@ -454,18 +484,18 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     on the inputs only (include/odise_b200.h states the error bound); the other two results are the same bits."""
     sfx = _msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
                         (grad_output, "grad_output")), im2col_step)
-    N, S, M, D, L, Lq, P = _msda_backward_shapes(value, sampling_loc, grad_output)
+    # value [N, S, M, D], sampling_loc [N, Lq, M, L, P, 2]
+    N, S, M, D = value.shape
+    _, Lq, _, L, P, _ = sampling_loc.shape
+    if grad_output.numel() != N * Lq * M * D:
+        raise OdiseError(f"grad_output: expected {N * Lq * M * D} elements, got {grad_output.numel()}")
     ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
     grad_value = torch.empty_like(value)
     grad_loc = torch.empty_like(sampling_loc)
     grad_attn = torch.empty_like(attn_weight)
-    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(sampling_loc), _ptr(attn_weight), _ptr(grad_output), _ptr(grad_value),
-            _ptr(grad_loc), _ptr(grad_attn), N, S, M, D, L, Lq, P)
-    if deterministic:
-        ws = _scratch(load().odise_msda_det_workspace_bytes(N, S, M, D), value.device)
-        _launch("odise_msda_backward_det_" + sfx, *args, _ptr(ws))
-    else:
-        _launch("odise_msda_backward_" + sfx, *args)
+    _launch(f"odise_msda_backward_{'det_' if deterministic else ''}{sfx}", value, ss, ls, sampling_loc, attn_weight,
+            grad_output, grad_value, grad_loc, grad_attn, N, S, M, D, L, Lq, P,
+            workspace=(lambda dll: dll.odise_msda_det_workspace_bytes(N, S, M, D)) if deterministic else None)
     return [grad_value, grad_loc, grad_attn]
 
 
@@ -480,8 +510,8 @@ def _msda_box(reference_points):
 def _msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output=None,
                      deterministic=False, dtypes=_FLOATS):
     """Checks of a fused MSDA call, the forward or (grad_output given) the backward, without data and without the
-    library (the fake implementations of odise_b200.msda's ops call it too): CUDA, contiguous, value of one of `dtypes`
-    and offsets, logits and grad_output of its dtype, reference_points float32, in the layouts of odise_msda_fused_f32
+    library: CUDA, contiguous, value of one of `dtypes` and offsets, logits and grad_output of its dtype,
+    reference_points float32, in the layouts of odise_msda_fused_f32
     (value [N, S, M, D], reference_points [N, Lq, L, 2] or boxes [N, Lq, L, 4] with a storage offset that keeps them
     16-byte aligned, offsets [N, Lq, M, L, P, 2], logits [N, Lq, M, L*P], grad_output [N, Lq, M*D]).  The 16-bit, the
     box and every backward entry point take D = 32, L*P <= 32 and S*M*D < 2^31 only (d32_ok in msda.cu; they return
@@ -522,8 +552,7 @@ def _msda_fused_forward(dtypes, value, spatial_shapes, level_start_index, refere
     ss, ls = _msda_index(value.device, spatial_shapes, level_start_index)
     out = torch.empty(N, Lq, M * D, dtype=value.dtype, device=value.device)
     planes = (None, None) if fn == "odise_msda_fused_f32" else ()    # its out_hi / out_lo, which only the engines use
-    _launch(fn, _ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(out),
-            *planes, N, S, M, D, L, Lq, P)
+    _launch(fn, value, ss, ls, reference_points, offsets, logits, out, *planes, N, S, M, D, L, Lq, P)
     return out
 
 
@@ -536,13 +565,9 @@ def _msda_fused_backward(dtypes, value, spatial_shapes, level_start_index, refer
     grad_value = torch.empty(value.shape, dtype=value.dtype if deterministic else torch.float32, device=value.device)
     grad_offs = torch.empty_like(offsets)
     grad_logits = torch.empty_like(logits)
-    args = (_ptr(value), _ptr(ss), _ptr(ls), _ptr(reference_points), _ptr(offsets), _ptr(logits), _ptr(grad_output),
-            _ptr(grad_value), _ptr(grad_offs), _ptr(grad_logits), N, S, M, D, L, Lq, P)
-    if deterministic:
-        ws = _scratch(load().odise_msda_det_workspace_bytes(N, S, M, D), value.device)
-        _launch(fn, *args, _ptr(ws))
-    else:
-        _launch(fn, *args)
+    _launch(fn, value, ss, ls, reference_points, offsets, logits, grad_output, grad_value, grad_offs, grad_logits,
+            N, S, M, D, L, Lq, P,
+            workspace=(lambda dll: dll.odise_msda_det_workspace_bytes(N, S, M, D)) if deterministic else None)
     if grad_value.dtype != value.dtype:
         grad_value = grad_value.to(value.dtype)
     return grad_value, grad_offs, grad_logits
@@ -594,8 +619,8 @@ def msda_fused_backward_16bit(value, spatial_shapes, level_start_index, referenc
 
 
 def _xattn_shapes(q, k, v, mask, heads, out=None, lse=None, grad_out=None):
-    """Checks of the masked cross-attention entry points, without data and without the library (the fake
-    implementations of odise_b200.masked_attn's ops call it too): q [Q, B, E], k and v [S, B, E], E = heads * 32, CUDA,
+    """Checks of the masked cross-attention entry points, without data and without the library: q [Q, B, E], k and v
+    [S, B, E], E = heads * 32, CUDA,
     contiguous, one dtype of float32 / float16 / bfloat16; mask None or a contiguous CUDA bool [B*heads, Q, S] or
     [Q, S]; for the backward out and grad_out like q and lse [B*heads, Q] float32.  -> (Q, B, E, S, mask_bh_stride)"""
     _tensor(q, "q", _FLOATS)
@@ -635,9 +660,8 @@ def masked_xattn_forward(q, k, v, mask, heads):
     Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads)
     out = torch.empty_like(q)
     lse = torch.empty(B * heads, Q, dtype=torch.float32, device=q.device)
-    ws = _scratch(load().odise_masked_xattn_workspace_bytes(B, heads, Q, S), q.device)
-    _launch("odise_masked_xattn_forward_" + _SFX[q.dtype], _ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out),
-            _ptr(lse), B, heads, 32, Q, S, _ptr(ws))
+    _launch("odise_masked_xattn_forward_" + _SFX[q.dtype], q, k, v, mask, stride, out, lse, B, heads, 32, Q, S,
+            workspace=lambda dll: dll.odise_masked_xattn_workspace_bytes(B, heads, Q, S))
     return out, lse
 
 
@@ -647,9 +671,8 @@ def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
     masked_xattn_forward, and for out / lse / grad_out of the wrong shape or dtype."""
     Q, B, E, S, stride = _xattn_shapes(q, k, v, mask, heads, out=out, lse=lse, grad_out=grad_out)
     gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-    ws = _scratch(load().odise_masked_xattn_workspace_bytes(B, heads, Q, S), q.device)
-    _launch("odise_masked_xattn_backward_" + _SFX[q.dtype], _ptr(q), _ptr(k), _ptr(v), _ptr(mask), stride, _ptr(out),
-            _ptr(lse), _ptr(grad_out), _ptr(gq), _ptr(gk), _ptr(gv), B, heads, 32, Q, S, _ptr(ws))
+    _launch("odise_masked_xattn_backward_" + _SFX[q.dtype], q, k, v, mask, stride, out, lse, grad_out, gq, gk, gv, B,
+            heads, 32, Q, S, workspace=lambda dll: dll.odise_masked_xattn_workspace_bytes(B, heads, Q, S))
     return gq, gk, gv
 
 
@@ -689,8 +712,7 @@ def mask_point_sample(maps, points):
         raise OdiseError(f"points: expected [{N}, P, 2], got {tuple(points.shape)}")
     _tensor(points, "points", torch.float32)
     out = torch.empty(N, points.shape[1], dtype=torch.float32, device=maps.device)
-    _launch("odise_mask_point_sample_" + _SFX[maps.dtype], _ptr(_u8(maps)), _ptr(points), _ptr(out), N, H, W,
-            points.shape[1])
+    _launch("odise_mask_point_sample_" + _SFX[maps.dtype], _u8(maps), points, out, N, H, W, points.shape[1])
     return out
 
 
@@ -718,8 +740,8 @@ def mask_cost(pred, prob, labels, tgt, points, counts, w_class, w_mask, w_dice, 
         out = torch.empty(B, Q, Tmax, dtype=torch.float32, device=pred.device)
     _tensor(out, "out", torch.float32, (B, Q, Tmax))
     cnt = (ctypes.c_int * B)(*counts)
-    _launch("odise_mask_cost_" + sfx, _ptr(pred), _ptr(prob), _ptr(labels), _ptr(_u8(tgt)), _ptr(points), cnt,
-            _ptr(out), B, Q, H, W, K1, Hg, Wg, Tmax, P, float(w_class), float(w_mask), float(w_dice))
+    _launch("odise_mask_cost_" + sfx, pred, prob, labels, _u8(tgt), points, cnt, out, B, Q, H, W, K1, Hg, Wg, Tmax, P,
+            float(w_class), float(w_mask), float(w_dice))
     return out
 
 
@@ -753,8 +775,8 @@ def mask_loss_forward(pred, tgt, pairs, cand, rnd, num_masks, num_points, k):
     # at least 16 bytes: the buffer is also the state mask_loss_backward takes, never empty
     ws = _scratch(max(load().odise_mask_loss_workspace_bytes(N, num_points), 16), pred.device)
     losses = torch.empty(2, dtype=torch.float32, device=pred.device)
-    _launch("odise_mask_loss_forward_" + sfx, _ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(cand), _ptr(rnd), _ptr(ws),
-            _ptr(losses), B, Q, H, W, Hg, Wg, N, num_points, S, k, float(num_masks))
+    _launch("odise_mask_loss_forward_" + sfx, pred, _u8(tgt), pairs, cand, rnd, ws, losses, B, Q, H, W, Hg, Wg, N,
+            num_points, S, k, float(num_masks))
     return losses, ws
 
 
@@ -768,8 +790,8 @@ def mask_loss_backward(pred, tgt, pairs, pair_of, state, grad_losses, num_masks,
     if not state.is_cuda or state.dtype != torch.uint8 or state.numel() < N * (16 + 8 * num_points):
         raise OdiseError("state: expected the workspace mask_loss_forward returned")
     grad = torch.empty_like(pred)
-    _launch("odise_mask_loss_backward_" + sfx, _ptr(pred), _ptr(_u8(tgt)), _ptr(pairs), _ptr(pair_of), _ptr(state),
-            _ptr(grad_losses), _ptr(grad), B, Q, H, W, Hg, Wg, N, num_points, float(num_masks))
+    _launch("odise_mask_loss_backward_" + sfx, pred, _u8(tgt), pairs, pair_of, state, grad_losses, grad, B, Q, H, W,
+            Hg, Wg, N, num_points, float(num_masks))
     return grad
 
 
@@ -777,9 +799,9 @@ MASK_HEAD_C, MASK_HEAD_MAX_Q = 256, 256    # the mask width and query count the 
 
 
 def _mask_head_shapes(embed, features, outputs_mask=None, weights=None, grad_mask=None, grad_pooled=None):
-    """Checks of the mask-head entry points, without data and without the library (the fake implementations of
-    odise_b200.decoder's ops call it too): embed [B, Q, 256] and features [B, 256, H, W] contiguous CUDA tensors of one
-    dtype of float32 / float16 / bfloat16, Q <= 256, H * W < 2^24; for the backward outputs_mask and grad_mask
+    """Checks of the mask-head entry points, without data and without the library: embed [B, Q, 256] and features
+    [B, 256, H, W] contiguous CUDA tensors of one dtype of float32 / float16 / bfloat16, Q <= 256, H * W < 2^24; for the
+    backward outputs_mask and grad_mask
     [B, Q, H, W] and grad_pooled [B, Q, 256] of that dtype and weights [B, Q] float32.  -> (suffix, B, Q, H, W)"""
     _tensor(embed, "mask_embed", _FLOATS)
     if embed.dim() != 3 or features.dim() != 4:
@@ -809,14 +831,15 @@ def mask_head_forward(embed, features, threshold=0.5):
     om = torch.empty(B, Q, H, W, dtype=embed.dtype, device=embed.device)
     pooled = torch.empty_like(embed)
     weights = torch.empty(B, Q, dtype=torch.float32, device=embed.device)
-    ws = _scratch(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W), embed.device)
-    _launch("odise_mask_head_forward_" + sfx, _ptr(embed), _ptr(features), _ptr(om), _ptr(pooled), _ptr(weights), B, Q,
-            MASK_HEAD_C, H, W, float(threshold), _ptr(ws))
+    _launch("odise_mask_head_forward_" + sfx, embed, features, om, pooled, weights, B, Q, MASK_HEAD_C, H, W,
+            float(threshold), workspace=lambda dll: dll.odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W))
     return om, pooled, weights
 
 
-def _mask_head_attn_shapes(outputs_mask, size, heads):
-    """Checks of mask_head_attn_mask (shared with its fake): -> (suffix, B, Q, H, W, h, w)"""
+def mask_head_attn_mask(outputs_mask, size, heads):
+    """The decoder's attention mask (odise_mask_head_attn_mask_*): outputs_mask [B, Q, H, W] -> bool
+    [B*heads, Q, h*w], True = blocked = sigmoid(bilinear resize to size = (h, w)) < 0.5 in torch's roundings for the
+    dtype, with every all-blocked row written all False (odise.py:683)."""
     _tensor(outputs_mask, "outputs_mask", _FLOATS)
     if outputs_mask.dim() != 4:
         raise OdiseError(f"outputs_mask must be [B, Q, H, W], got {tuple(outputs_mask.shape)}")
@@ -825,16 +848,8 @@ def _mask_head_attn_shapes(outputs_mask, size, heads):
     if min(B, Q, H, W, h, w, heads) <= 0 or B * Q >= 2 ** 31 or h * w >= 2 ** 31:
         raise OdiseError(f"attention mask: outputs_mask {tuple(outputs_mask.shape)}, size {(h, w)}, heads {heads} not "
                          "supported")
-    return _SFX[outputs_mask.dtype], B, Q, H, W, h, w
-
-
-def mask_head_attn_mask(outputs_mask, size, heads):
-    """The decoder's attention mask (odise_mask_head_attn_mask_*): outputs_mask [B, Q, H, W] -> bool
-    [B*heads, Q, h*w], True = blocked = sigmoid(bilinear resize to size = (h, w)) < 0.5 in torch's roundings for the
-    dtype, with every all-blocked row written all False (odise.py:683)."""
-    sfx, B, Q, H, W, h, w = _mask_head_attn_shapes(outputs_mask, size, heads)
     out = torch.empty(B * heads, Q, h * w, dtype=torch.bool, device=outputs_mask.device)
-    _launch("odise_mask_head_attn_mask_" + sfx, _ptr(outputs_mask), _ptr(out), B, Q, H, W, h, w, heads)
+    _launch("odise_mask_head_attn_mask_" + _SFX[outputs_mask.dtype], outputs_mask, out, B, Q, H, W, h, w, heads)
     return out
 
 
@@ -845,9 +860,9 @@ def mask_head_backward(embed, features, outputs_mask, weights, grad_mask, grad_p
     shape or dtype."""
     sfx, B, Q, H, W = _mask_head_shapes(embed, features, outputs_mask, weights, grad_mask, grad_pooled)
     ge, gx = torch.empty_like(embed), torch.empty_like(features)
-    ws = _scratch(load().odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W), embed.device)
-    _launch("odise_mask_head_backward_" + sfx, _ptr(embed), _ptr(features), _ptr(outputs_mask), _ptr(weights),
-            _ptr(grad_mask), _ptr(grad_pooled), _ptr(ge), _ptr(gx), B, Q, MASK_HEAD_C, H, W, float(threshold), _ptr(ws))
+    _launch("odise_mask_head_backward_" + sfx, embed, features, outputs_mask, weights, grad_mask, grad_pooled, ge, gx,
+            B, Q, MASK_HEAD_C, H, W, float(threshold),
+            workspace=lambda dll: dll.odise_mask_head_workspace_bytes(B, Q, MASK_HEAD_C, H, W))
     return ge, gx
 
 
@@ -857,9 +872,8 @@ CATEGORY_C_MULTIPLE, CATEGORY_MAX_C, CATEGORY_MAX_PROMPTS, CATEGORY_MAX_GROUP = 
 
 def _category_shapes(mask_embed, text_embed, null_embed, logit_scale, group_start, winners=None, norms=None,
                      grad_logits=None):
-    """Checks of the category-scoring entry points, without data and without the library (the fake implementations of
-    odise_b200.category's ops call it too): mask_embed [B, Q, C] float32 / float16 / bfloat16, text_embed [Kp, C] and
-    null_embed [1, C] of mask_embed's dtype or (16-bit mask_embed only) both float32, logit_scale a float32 scalar,
+    """Checks of the category-scoring entry points, without data and without the library: mask_embed [B, Q, C]
+    float32 / float16 / bfloat16, text_embed [Kp, C] and null_embed [1, C] of mask_embed's dtype or (16-bit mask_embed only) both float32, logit_scale a float32 scalar,
     group_start int32 [K + 1], all contiguous CUDA tensors; for the backward winners uint8 and grad_logits of
     mask_embed's dtype [B, Q, K + 1], norms float32 [B*Q + Kp + 1].  -> (suffix, bank_f32, B, Q, C, K, Kp)"""
     _tensor(mask_embed, "mask_embed", _FLOATS)
@@ -907,8 +921,8 @@ def category_logits_forward(mask_embed, text_embed, null_embed, logit_scale, gro
     out = torch.empty(B, Q, K + 1, dtype=mask_embed.dtype, device=dev)
     win = torch.empty(B, Q, K + 1, dtype=torch.uint8, device=dev)
     norms = torch.empty(B * Q + Kp + 1, dtype=torch.float32, device=dev)
-    _launch("odise_category_logits_forward_" + sfx, _ptr(mask_embed), _ptr(text_embed), _ptr(null_embed),
-            _ptr(logit_scale), _ptr(group_start), _ptr(out), _ptr(win), _ptr(norms), B * Q, C, K, Kp, bank_f32)
+    _launch("odise_category_logits_forward_" + sfx, mask_embed, text_embed, null_embed, logit_scale, group_start, out,
+            win, norms, B * Q, C, K, Kp, bank_f32)
     return out, win, norms
 
 
@@ -921,10 +935,9 @@ def category_logits_backward(mask_embed, text_embed, null_embed, logit_scale, gr
                                                      winners, norms, grad_logits)
     gm, gt, gn = torch.empty_like(mask_embed), torch.empty_like(text_embed), torch.empty_like(null_embed)
     gs = torch.empty((), dtype=torch.float32, device=mask_embed.device)
-    ws = _scratch(load().odise_category_logits_workspace_bytes(B * Q, C, K, Kp), mask_embed.device)
-    _launch("odise_category_logits_backward_" + sfx, _ptr(mask_embed), _ptr(text_embed), _ptr(null_embed),
-            _ptr(logit_scale), _ptr(group_start), _ptr(winners), _ptr(norms), _ptr(grad_logits), _ptr(gm), _ptr(gt),
-            _ptr(gn), _ptr(gs), B * Q, C, K, Kp, bank_f32, _ptr(ws))
+    _launch("odise_category_logits_backward_" + sfx, mask_embed, text_embed, null_embed, logit_scale, group_start,
+            winners, norms, grad_logits, gm, gt, gn, gs, B * Q, C, K, Kp, bank_f32,
+            workspace=lambda dll: dll.odise_category_logits_workspace_bytes(B * Q, C, K, Kp))
     return gm, gt, gn, gs
 
 
@@ -947,11 +960,12 @@ def _fpn_limits(N, C, h, w, H, W):
                          f"{FPN_C_MULTIPLE}, N * C / {FPN_C_MULTIPLE} <= 65535, H, h <= 65535, h*w*C < 2^31)")
 
 
-def _fpn_shapes(z, cur, size):
-    """Checks of fpn_upsample_add without data and without the library (the fake implementation in
-    odise_b200.pixel_decoder calls it too): z [N, h*w, C] float32 CUDA with channel-contiguous rows (strides
-    (>= h*w*C, C, 1); a token slice of the encoder's memory qualifies), cur [N, C, H, W] contiguous float32 CUDA.
-    -> (N, C, h, w, H, W, batch stride of z)"""
+def fpn_upsample_add(z, cur, size):
+    """The pixel decoder's FPN step (odise_fpn_upsample_add_f32): cur + F.interpolate(level, cur's H x W, "bilinear",
+    align_corners=False) of the level z [N, h*w, C] (token-major, read in place; size = (h, w)) -> y [N, C, H, W],
+    bit-equal to torch's CUDA result.  z is float32 CUDA with channel-contiguous rows (strides (>= h*w*C, C, 1); a
+    token slice of the encoder's memory qualifies), cur contiguous float32 CUDA.  OdiseError on CPU or non-float32
+    tensors, layouts and shapes the kernel does not take."""
     h, w = (int(s) for s in size)
     N, C, H, W = _fpn_nchw(cur, "cur")
     _tensor(z, "z", torch.float32, (N, h * w, C), contiguous=False)
@@ -959,35 +973,20 @@ def _fpn_shapes(z, cur, size):
     bs = z.stride(0) if N > 1 else h * w * C
     if z.stride(2) != 1 or (h * w > 1 and z.stride(1) != C) or bs < h * w * C:
         raise OdiseError(f"z: rows must be channel-contiguous with a batch stride >= h*w*C, got strides {z.stride()}")
-    return N, C, h, w, H, W, bs
-
-
-def fpn_upsample_add(z, cur, size):
-    """The pixel decoder's FPN step (odise_fpn_upsample_add_f32): cur + F.interpolate(level, cur's H x W, "bilinear",
-    align_corners=False) of the level z [N, h*w, C] (token-major, read in place; size = (h, w)) -> y [N, C, H, W],
-    bit-equal to torch's CUDA result.  OdiseError on CPU or non-float32 tensors, layouts and shapes the kernel does not
-    take."""
-    N, C, h, w, H, W, bs = _fpn_shapes(z, cur, size)
     y = torch.empty_like(cur)
-    _launch("odise_fpn_upsample_add_f32", _ptr(z), bs, _ptr(cur), _ptr(y), N, C, h, w, H, W)
+    _launch("odise_fpn_upsample_add_f32", z, bs, cur, y, N, C, h, w, H, W)
     return y
-
-
-def _fpn_backward_shapes(grad_y, size):
-    """Checks of fpn_upsample_add_backward (shared with its fake) -> (N, C, h, w, H, W)"""
-    h, w = (int(s) for s in size)
-    N, C, H, W = _fpn_nchw(grad_y, "grad_y")
-    _fpn_limits(N, C, h, w, H, W)
-    return N, C, h, w, H, W
 
 
 def fpn_upsample_add_backward(grad_y, size):
     """Backward of fpn_upsample_add for the level (odise_fpn_upsample_add_backward_f32): grad_y [N, C, H, W]
     contiguous float32 -> grad_z [N, h*w, C] contiguous, the adjoint of the bilinear resize, summed in a fixed order
     without atomics (bit-reproducible).  The gradient of cur is grad_y itself."""
-    N, C, h, w, H, W = _fpn_backward_shapes(grad_y, size)
+    h, w = (int(s) for s in size)
+    N, C, H, W = _fpn_nchw(grad_y, "grad_y")
+    _fpn_limits(N, C, h, w, H, W)
     gz = torch.empty(N, h * w, C, dtype=torch.float32, device=grad_y.device)
-    _launch("odise_fpn_upsample_add_backward_f32", _ptr(grad_y), _ptr(gz), h * w * C, N, C, h, w, H, W)
+    _launch("odise_fpn_upsample_add_backward_f32", grad_y, gz, h * w * C, N, C, h, w, H, W)
     return gz
 
 

@@ -23,38 +23,12 @@ from . import lib
 
 _DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 
-# The kernels as custom ops in the odise_b200 namespace.  As for the MSDA ops: the implementation is registered for every
-# device so that a CPU tensor reaches lib's own check, and the fakes refuse what lib refuses for reasons visible without
-# data.
-_OPS = torch.library.Library("odise_b200", "FRAGMENT")
-_OPS.define("masked_xattn_forward(Tensor q, Tensor k, Tensor v, Tensor? mask, int heads) -> (Tensor, Tensor)")
-_OPS.define("masked_xattn_backward(Tensor q, Tensor k, Tensor v, Tensor? mask, Tensor out, Tensor lse, "
-            "Tensor grad_out, int heads) -> (Tensor, Tensor, Tensor)")
-
-
-# lib's functions are looked up at call time, so that a test that patches them sees every call
-def _forward(q, k, v, mask, heads):
-    return lib.masked_xattn_forward(q, k, v, mask, heads)
-
-
-def _backward(q, k, v, mask, out, lse, grad_out, heads):
-    return lib.masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads)
-
-
-_OPS.impl("masked_xattn_forward", _forward, "CompositeExplicitAutograd")
-_OPS.impl("masked_xattn_backward", _backward, "CompositeExplicitAutograd")
-
-
-@torch.library.register_fake("odise_b200::masked_xattn_forward", lib=_OPS)
-def _forward_fake(q, k, v, mask, heads):
-    Q, B, E, S, _ = lib._xattn_shapes(q, k, v, mask, heads)
-    return torch.empty_like(q), q.new_empty(B * heads, Q, dtype=torch.float32)
-
-
-@torch.library.register_fake("odise_b200::masked_xattn_backward", lib=_OPS)
-def _backward_fake(q, k, v, mask, out, lse, grad_out, heads):
-    lib._xattn_shapes(q, k, v, mask, heads, out=out, lse=lse, grad_out=grad_out)
-    return torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+# The kernels as torch custom ops (lib.custom_op).  lib's functions are looked up at call time, so that a test that
+# patches them sees every call.
+lib.custom_op("masked_xattn_forward(Tensor q, Tensor k, Tensor v, Tensor? mask, int heads) -> (Tensor, Tensor)",
+              lambda *args: lib.masked_xattn_forward(*args))
+lib.custom_op("masked_xattn_backward(Tensor q, Tensor k, Tensor v, Tensor? mask, Tensor out, Tensor lse, "
+              "Tensor grad_out, int heads) -> (Tensor, Tensor, Tensor)", lambda *args: lib.masked_xattn_backward(*args))
 
 
 class MaskedCrossAttnFunction(Function):

@@ -28,27 +28,11 @@ from torch.autograd.function import once_differentiable
 from . import lib
 
 
-# The kernels as torch custom ops in namespace odise_b200, the one place where a traced graph (torch.compile,
-# torch.export) meets lib's ctypes calls, which Dynamo cannot trace.  The implementation is registered for every device,
-# so that a CPU tensor reaches lib's own check; the fake implementations give the results' shapes, dtypes and devices,
-# refuse what lib refuses for reasons visible without data (with lib's own validators) and never load the library.
-# torch.library.Library rather than torch.library.custom_op: its eager call goes straight to the dispatcher, without
-# custom_op's Python wrapper (DESIGN.md §3, "Under torch.compile").  There is no autograd formula on the ops: the Functions below are the
-# one autograd definition, and Dynamo traces them with the ops inside.
-_OPS = torch.library.Library("odise_b200", "FRAGMENT")
-_OPS.define("msda_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
-            "Tensor attn_weight, int im2col_step) -> Tensor")
-_OPS.define("msda_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
-            "Tensor attn_weight, Tensor grad_output, int im2col_step, bool deterministic) -> (Tensor, Tensor, Tensor)")
-_OPS.define("msda_fused_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
-            "Tensor reference_points, Tensor offsets, Tensor logits) -> Tensor")
-_OPS.define("msda_fused_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
-            "Tensor reference_points, Tensor offsets, Tensor logits, Tensor grad_output, bool deterministic) "
-            "-> (Tensor, Tensor, Tensor)")
 _LOW = (torch.float16, torch.bfloat16)
 
 
-# lib's functions are looked up at call time, so that a test that patches them sees every call
+# The kernels as torch custom ops (lib.custom_op).  lib's functions are looked up at call time, so that a test that
+# patches them sees every call.
 def _msda_forward(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
     fwd = lib.msda_forward_f64 if value.dtype == torch.float64 else lib.msda_forward
     return fwd(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step)
@@ -72,41 +56,16 @@ def _msda_fused_backward(value, spatial_shapes, level_start_index, reference_poi
                deterministic=deterministic)
 
 
-for _name, _fn in (("msda_forward", _msda_forward), ("msda_backward", _msda_backward),
-                   ("msda_fused_forward", _msda_fused_forward), ("msda_fused_backward", _msda_fused_backward)):
-    _OPS.impl(_name, _fn, "CompositeExplicitAutograd")
-
-
-@torch.library.register_fake("odise_b200::msda_forward", lib=_OPS)
-def _msda_forward_fake(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
-    lib._msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight")), im2col_step)
-    N, S, M, D = value.shape
-    _, Lq, _, L, P, _ = sampling_loc.shape
-    return value.new_empty(N, Lq, M * D)
-
-
-@torch.library.register_fake("odise_b200::msda_backward", lib=_OPS)
-def _msda_backward_fake(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, grad_output, im2col_step,
-                        deterministic):
-    lib._msda_inputs(((value, "value"), (sampling_loc, "sampling_loc"), (attn_weight, "attn_weight"),
-                      (grad_output, "grad_output")), im2col_step)
-    lib._msda_backward_shapes(value, sampling_loc, grad_output)
-    return torch.empty_like(value), torch.empty_like(sampling_loc), torch.empty_like(attn_weight)
-
-
-@torch.library.register_fake("odise_b200::msda_fused_forward", lib=_OPS)
-def _msda_fused_forward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits):
-    _, N, S, M, D, L, Lq, P = lib._msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets,
-                                                   logits)
-    return value.new_empty(N, Lq, M * D)
-
-
-@torch.library.register_fake("odise_b200::msda_fused_backward", lib=_OPS)
-def _msda_fused_backward_fake(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
-                              deterministic):
-    lib._msda_fused_call(value, spatial_shapes, level_start_index, reference_points, offsets, logits, grad_output,
-                         deterministic)
-    return torch.empty_like(value), torch.empty_like(offsets), torch.empty_like(logits)
+lib.custom_op("msda_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
+              "Tensor attn_weight, int im2col_step) -> Tensor", _msda_forward)
+lib.custom_op("msda_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, Tensor sampling_loc, "
+              "Tensor attn_weight, Tensor grad_output, int im2col_step, bool deterministic) -> (Tensor, Tensor, Tensor)",
+              _msda_backward)
+lib.custom_op("msda_fused_forward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
+              "Tensor reference_points, Tensor offsets, Tensor logits) -> Tensor", _msda_fused_forward)
+lib.custom_op("msda_fused_backward(Tensor value, Tensor spatial_shapes, Tensor level_start_index, "
+              "Tensor reference_points, Tensor offsets, Tensor logits, Tensor grad_output, bool deterministic) "
+              "-> (Tensor, Tensor, Tensor)", _msda_fused_backward)
 
 
 class MSDA:

@@ -37,34 +37,12 @@ from .decoder import PositionEmbeddingSine
 from .masked_attn import _activation
 from .msda import MSDeformAttn
 
-_OPS = torch.library.Library("odise_b200", "FRAGMENT")
-_OPS.define("fpn_upsample_add(Tensor z, Tensor cur, int h, int w) -> Tensor")
-_OPS.define("fpn_upsample_add_backward(Tensor grad_y, int h, int w) -> Tensor")
-
-
-# lib's functions are looked up at call time, so that a test that patches them sees every call
-def _forward(z, cur, h, w):
-    return lib.fpn_upsample_add(z, cur, (h, w))
-
-
-def _backward(grad_y, h, w):
-    return lib.fpn_upsample_add_backward(grad_y, (h, w))
-
-
-_OPS.impl("fpn_upsample_add", _forward, "CompositeExplicitAutograd")
-_OPS.impl("fpn_upsample_add_backward", _backward, "CompositeExplicitAutograd")
-
-
-@torch.library.register_fake("odise_b200::fpn_upsample_add", lib=_OPS)
-def _forward_fake(z, cur, h, w):
-    lib._fpn_shapes(z, cur, (h, w))
-    return torch.empty_like(cur)
-
-
-@torch.library.register_fake("odise_b200::fpn_upsample_add_backward", lib=_OPS)
-def _backward_fake(grad_y, h, w):
-    N, C, h, w, _, _ = lib._fpn_backward_shapes(grad_y, (h, w))
-    return grad_y.new_empty(N, h * w, C)
+# The kernels as torch custom ops (lib.custom_op).  lib's functions are looked up at call time, so that a test that
+# patches them sees every call.
+lib.custom_op("fpn_upsample_add(Tensor z, Tensor cur, int h, int w) -> Tensor",
+              lambda z, cur, h, w: lib.fpn_upsample_add(z, cur, (h, w)))
+lib.custom_op("fpn_upsample_add_backward(Tensor grad_y, int h, int w) -> Tensor",
+              lambda grad_y, h, w: lib.fpn_upsample_add_backward(grad_y, (h, w)))
 
 
 class FpnUpsampleAddFunction(Function):
