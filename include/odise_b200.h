@@ -42,6 +42,8 @@ extern "C" {
 #define ODISE_ACT_SILU 2
 #define ODISE_ACT_GELU 3
 #define ODISE_ACT_QUICKGELU 4 /* x * sigmoid(1.702 x): open_clip QuickGELU (CLIP ViT MLP) */
+/* Every entry point that takes an `act` (odise_gemm_bf16, the groupnorm apply passes, odise_act_split_f32) implements
+ * these five codes and returns ODISE_ERR_ARG for any other. */
 
 /* operand-plane formats (see the convention above) */
 #define ODISE_PLANES_BF16 0   /* (hi, lo) bf16 pair */
@@ -238,7 +240,7 @@ typedef struct odise_gemm_desc {
   float alpha;
   const float* bias;                 /* [N] or NULL */
   const float* rowbias; int rows_per_group; long long rowbias_ld; /* [groups, N] or NULL */
-  int act;
+  int act;                           /* ODISE_ACT_* (any other code: ODISE_ERR_ARG) */
   const float* residual; long long ld_residual; long long residual_batch_stride;
   float* out_f32; long long ld_out; long long out_batch_stride;
   void* out_hi; void* out_lo; long long ld_out_bf16; long long out_bf16_batch_stride;
@@ -297,7 +299,8 @@ int odise_groupnorm_stats_ws_f32(const float* x, long long ldx, long long x_bs, 
  * over the activation (odise_groupnorm_stats_ws_f32) when the activation was produced by our own GEMM. */
 int odise_groupnorm_finalize_seg_f32(const float* partial, long long seg_stride, long long plane_stride, float* mean,
                                      float* rstd, int B, int HW, int C, int G, float eps, void* stream);
-/* y = act(gn(x) * gamma + beta): writes fp32 (optional) and (hi, lo) planes (optional). act: NONE/SILU/RELU.
+/* y = act(gn(x) * gamma + beta): writes fp32 (optional) and (hi, lo) planes (optional).
+ * act: NONE / RELU / SILU / GELU / QUICKGELU (ODISE_ACT_*); any other code returns ODISE_ERR_ARG.
  * The *_bs variants take explicit per-image strides (elements; 0 = dense) so a level can be read from / written
  * into the level-concatenated [B, S, C] token matrix of the pixel decoder (msdeformattn.py:61-78). */
 int odise_groupnorm_apply_f32(const float* x, long long ldx, const float* mean, const float* rstd,
@@ -333,7 +336,7 @@ int odise_geglu_f32(const float* x, long long ldx, void* hi, void* lo, long long
 /* y = a + b (optional b, optional fp32 y) -> (hi, lo); b_rows > 0 broadcasts b over rows modulo b_rows */
 int odise_add_split_f32(const float* a, long long lda, const float* b, long long ldb, long long b_rows, float* y,
                         long long ldy, void* hi, void* lo, long long ldo, long long rows, int cols, void* stream);
-/* y = act(x) -> (hi, lo)  (SiLU(emb) in front of ResBlock.emb_layers) */
+/* y = act(x) -> (hi, lo)  (SiLU(emb) in front of ResBlock.emb_layers); act: an ODISE_ACT_* code, else ODISE_ERR_ARG */
 int odise_act_split_f32(const float* x, long long ldx, int act, void* hi, void* lo, long long ldo, long long rows,
                         int cols, void* stream);
 /* nearest 2x upsample of NHWC x[B,H,W,C] -> (hi, lo) [B,2H,2W,C] (ldm Upsample before its conv3x3) */

@@ -31,8 +31,12 @@ __device__ __forceinline__ float act_apply(float v, int act) {
   // (25 instr / element, ncu r1f); 1e-6 relative is far inside the 1e-3 parity budget
   if (act == ODISE_ACT_SILU) return __fdividef(v, 1.f + __expf(-v));
   if (act == ODISE_ACT_GELU) return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+  if (act == ODISE_ACT_QUICKGELU) return v / (1.f + __expf(-1.702f * v));   // the GEMM epilogue's expression (gemm_tc.cu)
   return v;
 }
+
+// the activation codes act_apply implements; every entry point taking `act` refuses any other with ODISE_ERR_ARG
+static inline bool act_ok(int act) { return act >= ODISE_ACT_NONE && act <= ODISE_ACT_QUICKGELU; }
 
 __device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* lo, float4 v) {
   const float e[4] = {v.x, v.y, v.z, v.w};
@@ -1049,7 +1053,7 @@ extern "C" int odise_groupnorm_apply_bs_f32(const float* x, long long ldx, long 
                                             const float* rstd, const float* gamma, const float* beta, int act,
                                             float* y, long long ldy, long long y_bs, void* hi, void* lo,
                                             long long ldo, long long o_bs, int B, int HW, int C, int G, void* stream) {
-  if (!x || !mean || !rstd || !gamma || !beta || (!y && !hi) || C % G) return ODISE_ERR_ARG;
+  if (!x || !mean || !rstd || !gamma || !beta || (!y && !hi) || C % G || !act_ok(act)) return ODISE_ERR_ARG;
   if (C % 4 || ldx % 4 || x_bs % 4 || (y && (ldy % 4 || y_bs % 4)) || (hi && (ldo % 4 || o_bs % 4)))
     return ODISE_ERR_ALIGN;
   Q8_CHECK(lo, ldo);
@@ -1223,7 +1227,7 @@ extern "C" int odise_softmax_split_f32(const float* x, long long ldx, void* hi, 
 
 extern "C" int odise_act_split_f32(const float* x, long long ldx, int act, void* hi, void* lo, long long ldo,
                                    long long rows, int cols, void* stream) {
-  if (!x || !hi || rows <= 0 || cols <= 0) return ODISE_ERR_ARG;
+  if (!x || !hi || rows <= 0 || cols <= 0 || !act_ok(act)) return ODISE_ERR_ARG;
   if (cols % 4 || ldx % 4 || ldo % 4) return ODISE_ERR_ALIGN;
   Q8_CHECK(lo, ldo);
   act_split_kernel<<<grid_for(rows * (cols / 4), 256), 256, 0, STREAM(stream)>>>(x, ldx, act, BF(hi), BFL(lo), ldo,
@@ -1237,7 +1241,7 @@ extern "C" int odise_groupnorm_apply_res_f32(const float* x, long long ldx, cons
                                              long long ldres, int act, float* y, long long ldy, int accumulate,
                                              void* hi, void* lo, long long ldo, int B, int HW, int C, int G,
                                              void* stream) {
-  if (!x || !mean || !rstd || !gamma || !beta || (!y && !hi) || C % G) return ODISE_ERR_ARG;
+  if (!x || !mean || !rstd || !gamma || !beta || (!y && !hi) || C % G || !act_ok(act)) return ODISE_ERR_ARG;
   if (C % 4 || ldx % 4 || (y && ldy % 4) || (hi && ldo % 4) || (res && ldres % 4)) return ODISE_ERR_ALIGN;
   Q8_CHECK(lo, ldo);
   int rc = launch_gn_apply(x, ldx, mean, rstd, gamma, beta, act, y, ldy, BF(hi), BFL(lo), ldo, B, HW, C, G,

@@ -686,6 +686,7 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
   if (d->nmma != 1 && (!d->a_lo || !d->b_lo)) return ODISE_ERR_ARG;
   if (d->M <= 0 || d->N <= 0 || d->K <= 0 || d->batch <= 0) return ODISE_ERR_ARG;
   if (!d->out_f32 && !d->out_hi) return ODISE_ERR_ARG;
+  if (d->act < ODISE_ACT_NONE || d->act > ODISE_ACT_QUICKGELU) return ODISE_ERR_ARG;   // the codes apply_act implements
 
   GemmParams p{};
   p.M = d->M; p.N = d->N; p.K = d->K; p.batch = d->batch;

@@ -37,7 +37,7 @@ def test_gemm_plain(cuda, nmma, bn, mnk):
         assert _rel(ap.float(), a) < 1e-4
 
 
-@pytest.mark.parametrize("act", [0, 1, 2, 3])
+@pytest.mark.parametrize("act", [0, 1, 2, 3, 4])
 def test_gemm_epilogue(cuda, act):
     from odise_b200 import lib
     M, N, K, G = 512, 256, 192, 4
@@ -47,7 +47,7 @@ def test_gemm_epilogue(cuda, act):
     out = torch.empty(M, N, device=cuda)
     lib.gemm(lib.split(a), lib.split(b), alpha=0.5, rowbias=rb, rows_per_group=M // G, act=act, out=out)
     ref = 0.5 * (a.double() @ b.double().t()) + rb.double().repeat_interleave(M // G, 0)
-    ref = [lambda x: x, F.relu, F.silu, F.gelu][act](ref)
+    ref = [lambda x: x, F.relu, F.silu, F.gelu, lambda x: x * torch.sigmoid(1.702 * x)][act](ref)   # 4: QuickGELU
     assert _rel(out, ref) < 2e-5
 
 
