@@ -657,6 +657,53 @@ int odise_category_logits_backward_bf16(const void* mask_embed, const void* text
                                         int C, int K, int Kp, int bank_f32, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Grounding loss for training (odise.py:779-907 MaskGroundingCriterion.get_loss) for S prediction sets at once:
+ * mask_embed [S, G, Q, C] and word_embed [G, K, C] are the G gathered images of the step (G = B on one rank), the B
+ * local ones at rows offset .. offset + B - 1; word_valid uint8 [G, K] (bool); logit_scale float32 [S] on the device.
+ * All tensors contiguous.  _f32 / _f16 / _bf16: mask_embed and its gradients in float, __half or __nv_bfloat16;
+ * word_embed and its gradients in the same type, or in float when words_f32 = 1 (float32 words under autocast; ignored
+ * by _f32).  All arithmetic fp32; in 16 bits the normalised rows, the dot products and logit_scale are rounded to the
+ * storage type where torch's autocast rounds them, and the scaled product is rounded once.
+ * odise_grounding_forward_*: losses float32 [S] = loss_weight (l1 + l2) / 2 per set, with the reference's fallback for
+ *   a non-finite l2 taken on the device; state float32 [S*G*Q*C + G*K*C + S*G*Q + G*K + 4*S*G*B] (the normalised rows,
+ *   their clamped norms, the two score matrices and the unit gradients of the loss against them), read by the backward.
+ * odise_grounding_backward_*: from the forward's inputs and state and grad_losses float32 [S]: the mask gradient
+ *   through the local-mask scores grad_mask_local [S, B, Q, C] and through the gathered-mask scores grad_mask_global
+ *   [S, G, Q, C], the word gradient through the local-word scores grad_word_local [B, K, C] and through the
+ *   gathered-word scores grad_word_global [G, K, C], and grad_logit_scale float32 [S].  workspace:
+ *   odise_grounding_workspace_bytes(...) bytes, 4-byte aligned, any content (0 for shapes the entry points refuse).
+ *   It holds the per-pair tiles and the partial sums over fixed chunks of partners, added in chunk order without
+ *   atomics: every gradient is bit-reproducible.
+ * Limits: 1 <= B <= G, 0 <= offset <= G - B, Q <= 256, 1 <= K <= 32, C a multiple of 32 up to 768, S*G*Q*C < 2^31
+ * (ODISE_ERR_UNSUPPORTED otherwise).  Three launches forward and three backward.  No host synchronisation and no
+ * allocation (CUDA-graph capturable). */
+long long odise_grounding_workspace_bytes(int S, int G, int B, int offset, int Q, int K, int C);
+int odise_grounding_forward_f32(const void* mask_embed, const void* word_embed, const uint8_t* word_valid,
+                                const float* logit_scale, float* losses, float* state, int S, int G, int B, int offset,
+                                int Q, int K, int C, float loss_weight, int words_f32, void* stream);
+int odise_grounding_forward_f16(const void* mask_embed, const void* word_embed, const uint8_t* word_valid,
+                                const float* logit_scale, float* losses, float* state, int S, int G, int B, int offset,
+                                int Q, int K, int C, float loss_weight, int words_f32, void* stream);
+int odise_grounding_forward_bf16(const void* mask_embed, const void* word_embed, const uint8_t* word_valid,
+                                 const float* logit_scale, float* losses, float* state, int S, int G, int B, int offset,
+                                 int Q, int K, int C, float loss_weight, int words_f32, void* stream);
+int odise_grounding_backward_f32(const void* mask_embed, const void* word_embed, const float* logit_scale,
+                                 const float* state, const float* grad_losses, void* grad_mask_local,
+                                 void* grad_mask_global, void* grad_word_local, void* grad_word_global,
+                                 float* grad_logit_scale, int S, int G, int B, int offset, int Q, int K, int C,
+                                 int words_f32, void* workspace, void* stream);
+int odise_grounding_backward_f16(const void* mask_embed, const void* word_embed, const float* logit_scale,
+                                 const float* state, const float* grad_losses, void* grad_mask_local,
+                                 void* grad_mask_global, void* grad_word_local, void* grad_word_global,
+                                 float* grad_logit_scale, int S, int G, int B, int offset, int Q, int K, int C,
+                                 int words_f32, void* workspace, void* stream);
+int odise_grounding_backward_bf16(const void* mask_embed, const void* word_embed, const float* logit_scale,
+                                  const float* state, const float* grad_losses, void* grad_mask_local,
+                                  void* grad_mask_global, void* grad_word_local, void* grad_word_global,
+                                  float* grad_logit_scale, int S, int G, int B, int offset, int Q, int K, int C,
+                                  int words_f32, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask head helpers (odise.py:937-963 MaskPooling, odise.py:746 einsum) */
 /* mask_logits [B, Q, HW] fp32 -> binary (logit > 0) as bf16 plane [B, Q, HWpad] + counts [B, Q] */
 int odise_mask_binarize_f32(const float* logits, void* bin_bf16, long long ld_bin, float* counts, int B, int Q,

@@ -941,6 +941,84 @@ def category_logits_backward(mask_embed, text_embed, null_embed, logit_scale, gr
     return gm, gt, gn, gs
 
 
+# the grounding-loss kernels' limits: Q up to 256 queries, 1..32 words, C a multiple of 32 up to 768
+GROUNDING_MAX_Q, GROUNDING_MAX_K, GROUNDING_C_MULTIPLE, GROUNDING_MAX_C = 256, 32, 32, 768
+
+
+def _grounding_shapes(mask_embed, word_embed, logit_scale, batch, offset, word_valid=None, state=None,
+                      grad_losses=None):
+    """Checks of the grounding-loss entry points, without data and without the library: mask_embed [S, G, Q, C]
+    float32 / float16 / bfloat16, word_embed [G, K, C] of mask_embed's dtype or (16-bit mask_embed only) float32,
+    logit_scale float32 [S], 1 <= batch <= G, 0 <= offset <= G - batch, all contiguous CUDA tensors; word_valid bool
+    [G, K], state float32 [grounding_state_size(...)], grad_losses float32 [S].
+    -> (suffix, words_f32, S, G, Q, K, C)"""
+    _tensor(mask_embed, "mask_embed", _FLOATS)
+    if mask_embed.dim() != 4 or word_embed.dim() != 3:
+        raise OdiseError(f"mask_embed must be [S, G, Q, C] and word_embed [G, K, C], got {tuple(mask_embed.shape)} and "
+                         f"{tuple(word_embed.shape)}")
+    S, G, Q, C = mask_embed.shape
+    K = word_embed.shape[1]
+    if not 0 <= offset <= G - batch or not grounding_supported(S, G, batch, Q, K, C):
+        raise OdiseError(f"grounding loss: S = {S}, G = {G}, B = {batch}, offset = {offset}, Q = {Q}, K = {K}, C = {C} "
+                         f"not supported (1 <= B <= G, Q <= {GROUNDING_MAX_Q}, 1 <= K <= {GROUNDING_MAX_K}, C a "
+                         f"multiple of {GROUNDING_C_MULTIPLE} up to {GROUNDING_MAX_C})")
+    _tensor(word_embed, "word_embed", (mask_embed.dtype, torch.float32), (G, K, C))     # float32 words under autocast
+    _tensor(logit_scale, "logit_scale", torch.float32, (S,))
+    if word_valid is not None:
+        _tensor(word_valid, "word_valid", torch.bool, (G, K))
+    if state is not None:
+        _tensor(state, "state", torch.float32, (grounding_state_size(S, G, batch, Q, K, C),))
+    if grad_losses is not None:
+        _tensor(grad_losses, "grad_losses", torch.float32, (S,))
+    return _SFX[mask_embed.dtype], int(word_embed.dtype != mask_embed.dtype), S, G, Q, K, C
+
+
+def grounding_supported(S, G, B, Q, K, C):
+    """whether the grounding kernels take S sets of G gathered images (B local), Q queries, K words, C channels: the
+    limits above and 32-bit element counts of the gathered masks, the words and the backward's per-pair tiles"""
+    P = B * (2 * G - B)     # (mask image, word image) pairs with the mask or the word image local
+    return (min(S, Q) > 0 and 1 <= B <= G and Q <= GROUNDING_MAX_Q and 1 <= K <= GROUNDING_MAX_K
+            and C % GROUNDING_C_MULTIPLE == 0 and 0 < C <= GROUNDING_MAX_C and S * G * Q * C < 2 ** 31
+            and S * P * Q * K < 2 ** 31 and G * K * C < 2 ** 31)
+
+
+def grounding_state_size(S, G, B, Q, K, C):
+    """float32 elements of the grounding forward's state (include/odise_b200.h)"""
+    return S * G * Q * C + G * K * C + S * G * Q + G * K + 4 * S * G * B
+
+
+def grounding_forward(mask_embed, word_embed, word_valid, logit_scale, batch, offset, loss_weight):
+    """MaskGroundingCriterion.get_loss for S prediction sets (odise_grounding_forward_* by mask_embed's dtype) on the
+    gathered mask_embed [S, G, Q, C], word_embed [G, K, C] and word_valid [G, K], this rank's `batch` images at rows
+    offset .. offset + batch - 1 -> (losses float32 [S], state float32, read by grounding_backward).  OdiseError on
+    CPU, non-contiguous or mixed-dtype tensors and on shapes the kernels do not take."""
+    sfx, wf32, S, G, Q, K, C = _grounding_shapes(mask_embed, word_embed, logit_scale, batch, offset, word_valid)
+    dev = mask_embed.device
+    losses = torch.empty(S, dtype=torch.float32, device=dev)
+    state = torch.empty(grounding_state_size(S, G, batch, Q, K, C), dtype=torch.float32, device=dev)
+    _launch("odise_grounding_forward_" + sfx, mask_embed, word_embed, word_valid, logit_scale, losses, state, S, G,
+            batch, offset, Q, K, C, float(loss_weight), wf32)
+    return losses, state
+
+
+def grounding_backward(mask_embed, word_embed, logit_scale, state, grad_losses, batch, offset):
+    """Backward of grounding_forward (odise_grounding_backward_*) -> (grad_mask_local [S, B, Q, C], grad_mask_global
+    [S, G, Q, C], grad_word_local [B, K, C], grad_word_global [G, K, C], grad_logit_scale float32 [S]): the gradients
+    through the uses of the local and of the gathered rows, kept apart for the caller to combine; each in its input's
+    dtype.  Fixed-order sums without atomics, so every gradient is bit-reproducible."""
+    sfx, wf32, S, G, Q, K, C = _grounding_shapes(mask_embed, word_embed, logit_scale, batch, offset, None, state,
+                                                 grad_losses)
+    gml = mask_embed.new_empty(S, batch, Q, C)
+    gmg = torch.empty_like(mask_embed)
+    gwl = word_embed.new_empty(batch, K, C)
+    gwg = torch.empty_like(word_embed)
+    gs = torch.empty_like(logit_scale)
+    _launch("odise_grounding_backward_" + sfx, mask_embed, word_embed, logit_scale, state, grad_losses, gml, gmg, gwl,
+            gwg, gs, S, G, batch, offset, Q, K, C, wf32,
+            workspace=lambda dll: dll.odise_grounding_workspace_bytes(S, G, batch, offset, Q, K, C))
+    return gml, gmg, gwl, gwg, gs
+
+
 FPN_C_MULTIPLE = 32     # the FPN upsample-add kernels take C a multiple of this
 
 
