@@ -118,7 +118,7 @@ class BackboneEngine:
     # ------------------------------------------------------------------------------------------- pieces
     def conditioning(self, clip_embed, B):
         """-> (context [B*77, 768], cond_emb [B, 1280])"""
-        e_p = ops.split(clip_embed, lo=self.lo)
+        e_p = lib.split(clip_embed, lo=self.lo)
         proj = ops.empty(B, 768, self.dev)
         lib.gemm(e_p, self.W["clip_project"], nmma=self.nmma, bias=self.F["clip_project.b"], out=proj)
         ctx = ops.bcast_fma(self.F["cond.a0"], self.F["cond.ta"], proj, B, CTX_T, 768)
@@ -155,7 +155,7 @@ class BackboneEngine:
                 x = ops.resize_nhwc(x, B, h, w, th, tw, bilinear=False)       # F.interpolate default = nearest
             M = B * th * tw
             n = f"p{idx}."
-            x_p = ops.split(x, lo=self.lo)
+            x_p = lib.split(x, lo=self.lo)
             # every conv leaves the GroupNorm records of its output in its epilogue (lib.GnStats): no statistics passes
             t1, s1 = ops.empty(M, 128, self.dev), lib.GnStats(M, 128, self.dev)
             lib.gemm(x_p, self.W[n + "c1"], nmma=self.nmma, out=t1, gn=s1)

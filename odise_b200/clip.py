@@ -292,7 +292,7 @@ class ClipTextEngine:
         eot = (token_ids.cpu().argmax(dim=-1) + torch.arange(N) * TS).to(torch.int32).to(dev)      # clip.py:150
         rows = ops.gather_rows(x, eot)
         out = ops.empty(N, self.proj.rows, dev)
-        lib.gemm(ops.split(rows, lo=self.lo), self.proj, nmma=self.nmma, out=out)
+        lib.gemm(lib.split(rows, lo=self.lo), self.proj, nmma=self.nmma, out=out)
         return out, enc
 
 

@@ -190,10 +190,10 @@ class HeadEngine:
         for i, n in enumerate(names):
             x, h, w = feats[n]
             t, ts = ops.empty(B * h * w, 256, dev), lib.GnStats(B * h * w, 256, dev)
-            self._gemm(ops.split(x, lo=self.lo), f"pd.in{i}", out=t, gn=ts)
+            self._gemm(lib.split(x, lo=self.lo), f"pd.in{i}", out=t, gn=ts)
             ops.group_norm(t, B, h * w, self.F[f"pd.in{i}.gn.g"], self.F[f"pd.in{i}.gn.be"], 1e-5, want_planes=False,
                            y=src[starts[i]:], ldy=256, y_bs=S * 256, stats=ts)
-        src_p = ops.split(src, lo=self.lo)
+        src_p = lib.split(src, lo=self.lo)
         for l in range(self.n_enc):
             n = f"pd.l{l}."
             _, q_p = ops.add_split(src, g["pd_pos"], b_rows=S, lo=self.lo)
@@ -217,12 +217,12 @@ class HeadEngine:
         x2, h2, w2 = feats["s2"]
         h3, w3 = shapes[2]
         lat, lat_s = ops.empty(B * h2 * w2, 256, dev), lib.GnStats(B * h2 * w2, 256, dev)
-        self._gemm(ops.split(x2, lo=self.lo), "pd.adapter", bias=False, out=lat, gn=lat_s)
+        self._gemm(lib.split(x2, lo=self.lo), "pd.adapter", bias=False, out=lat, gn=lat_s)
         cur, _ = ops.group_norm(lat, B, h2 * w2, self.F["pd.adapter.gn.g"], self.F["pd.adapter.gn.be"], 1e-5,
                                 want_f32=True, want_planes=False, stats=lat_s)
         ops.resize_nhwc(src[starts[2]:], B, h3, w3, h2, w2, True, dst=cur, accumulate=True, src_bs=S * 256)
         conv, conv_s = ops.empty(B * h2 * w2, 256, dev), lib.GnStats(B * h2 * w2, 256, dev)
-        self._gemm(ops.split(cur, lo=self.lo), "pd.layer", bias=False, M=B * h2 * w2, N=256, conv=(256, h2, w2), out=conv,
+        self._gemm(lib.split(cur, lo=self.lo), "pd.layer", bias=False, M=B * h2 * w2, N=256, conv=(256, h2, w2), out=conv,
                    gn=conv_s)
         _, y2_p = ops.group_norm(conv, B, h2 * w2, self.F["pd.layer.gn.g"], self.F["pd.layer.gn.be"], 1e-5, ACT_RELU,
                                  lo=self.lo, stats=conv_s)
@@ -252,12 +252,12 @@ class HeadEngine:
         h2, w2 = int(mask_features.shape[2]), int(mask_features.shape[3])
         HW = h2 * w2
         mf = ops.nchw_to_nhwc(mask_features.float())                       # [B*HW, 256]
-        mf_p = ops.split(mf, lo=self.lo)
+        mf_p = lib.split(mf, lo=self.lo)
         mft = ops.empty(256, B * HW, dev)                                  # [C, B*HW]: image z at column offset z*HW
         src = mask_features.float().contiguous().view(B, 256, HW)
         for z in range(B):
             ops.copy2d(src[z], mft[:, z * HW:(z + 1) * HW])
-        mft_p = ops.split(mft, lo=self.lo)
+        mft_p = lib.split(mft, lo=self.lo)
         return dict(memory=mem, memory_p=None, shapes=shapes, geo=g, mf_p=mf_p, mft_p=mft_p, mf=mf, mask_hw=(h2, w2))
 
     # ------------------------------------------------------------------------------------------- decoder
@@ -371,7 +371,7 @@ class HeadEngine:
             output, _ = self._ln(t, n + "cn", want_f32=True, want_planes=False)
             # self-attention
             _, qk_p = ops.add_split(output, qe, b_rows=Q, lo=self.lo)
-            out_p = ops.split(output, lo=self.lo)
+            out_p = lib.split(output, lo=self.lo)
             qkv = ops.empty(B * Q, 768, dev)
             self._gemm(qk_p, n + "sqk", out=qkv[:, :512], ld_out=768)
             self._gemm(out_p, n + "sv", out=qkv[:, 512:], ld_out=768)
@@ -397,9 +397,9 @@ class HeadEngine:
         dev = self.dev
         tb = self._f(text_bank)
         te = ops.empty(tb.shape[0], 256, dev)
-        self._gemm(ops.split(tb, lo=self.lo), "cat.text_proj", out=te)
+        self._gemm(lib.split(tb, lo=self.lo), "cat.text_proj", out=te)
         ne = ops.empty(1, 256, dev)
-        self._gemm(ops.split(self._f(null_bank).view(1, -1), lo=self.lo), "cat.text_proj", out=ne)
+        self._gemm(lib.split(self._f(null_bank).view(1, -1), lo=self.lo), "cat.text_proj", out=ne)
         gs = torch.zeros(len(group_sizes) + 1, dtype=torch.int32)
         gs[1:] = torch.as_tensor(group_sizes, dtype=torch.int32).cumsum(0)
         self._vocab[key] = dict(te=te, ne=ne, te_p=ops.l2_normalize_split(te, lo=self.lo),

@@ -116,8 +116,10 @@ _Tensor = torch.Tensor
 
 def _launch(name, *args, workspace=None):
     """Run entry point `name` on the current stream; OdiseError if it returns an error code.  Tensor arguments are
-    passed as their addresses; ints, floats, None and ctypes arrays as they are.  workspace, if given, maps the loaded
-    library to a byte count: a _scratch buffer of that size on the first argument's device goes last."""
+    passed as their addresses; ints, floats, None, ctypes arrays and byref() as they are.  workspace, if given, maps the
+    loaded library to a byte count: a _scratch buffer of that size on the first argument's device goes last.
+    Every entry point that takes a stream is called through here; host-only calls, which take none (the workspace size
+    queries, odise_gemm_tile_policy, odise_set_operand_format, the launch counter, profile_*), call load() directly."""
     if _NO_LAUNCH.get():
         return
     dll = load()
@@ -303,13 +305,11 @@ def split(x, out=None, lo=True, f16=False):
     if out is None:
         out = Planes.empty(rows, cols, x.device, lo=lo, f16=f16)
     if out.f16:
-        _check(load().odise_split_f16_f32(_ptr(x2), x2.stride(0), _ptr(out.hi), _ptr(out.lo), out.ld, rows, cols, _stream()),
-               "odise_split_f16_f32")
+        _launch("odise_split_f16_f32", x2, x2.stride(0), out.hi, out.lo, out.ld, rows, cols)
     else:
         if out.fmt == "q8" and cols % 4:
             raise OdiseError("split: F16Q8 planes need cols % 4 == 0")
-        hi, lo_p, ld = pargs(out)
-        _check(load().odise_split_f32(_ptr(x2), x2.stride(0), hi, lo_p, ld, rows, cols, _stream()), "odise_split_f32")
+        _launch("odise_split_f32", x2, x2.stride(0), *pargs(out), rows, cols)
     return out
 
 
@@ -418,7 +418,7 @@ def gemm(a, b, *, M=None, N=None, K=None, nmma=3, batch=1, a_bs=0, b_bs=0, conv=
             d.gn_seg_stride, d.gn_plane_stride = 3 * gn.Ctot, gn.Ctot
     d.geglu = 1 if geglu else 0
     d.conv_mode = conv_mode
-    _check(load().odise_gemm_bf16(ctypes.byref(d), _stream()), "odise_gemm_bf16")
+    _launch("odise_gemm_bf16", ctypes.byref(d))
     return out if out is not None else out_planes
 
 

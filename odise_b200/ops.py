@@ -1,9 +1,10 @@
 """Thin typed wrappers over the C ABI used by the engines (unet.py, head.py).  Activations are token-major /
-NHWC fp32 matrices [rows, C]; GEMM operands are lib.Planes.  No torch math on the hot path: torch only allocates."""
+NHWC fp32 matrices [rows, C]; GEMM operands are lib.Planes.  No torch math on the hot path: torch only allocates.
+Every launch goes through lib._launch, which passes tensors as their addresses and the current stream last."""
 import torch
 
 from . import lib
-from .lib import Planes, _check, _ptr, _stream, load
+from .lib import Planes
 
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_GELU, ACT_QUICKGELU = 0, 1, 2, 3, 4
 
@@ -12,23 +13,18 @@ def empty(rows, cols, device):
     return torch.empty(rows, cols, dtype=torch.float32, device=device)
 
 
-def split(x, lo=True):
-    return lib.split(x, lo=lo)
-
-
-def _gn_stats(L, x, ldx, x_bs, mean, rstd, B, HW, C, G, eps):
-    ws = torch.empty(int(L.odise_groupnorm_ws_floats(B, HW, C, G)), dtype=torch.float32, device=x.device)
-    _check(L.odise_groupnorm_stats_ws_f32(_ptr(x), ldx, x_bs, _ptr(ws), _ptr(mean), _ptr(rstd), B, HW, C, G, eps,
-                                          _stream()), "groupnorm_stats")
-
-
-def _gn_stats_any(L, x, ldx, x_bs, mean, rstd, B, HW, C, G, eps, stats):
-    """statistics from the producer epilogues' records when they exist, else the stand-alone pass over x"""
+def _gn_stats(x, ldx, x_bs, B, HW, C, G, eps, stats):
+    """-> (mean, rstd) [B*G] of x's groups: from the producer epilogues' records when they exist, else from the
+    stand-alone pass over x"""
+    mean = torch.empty(B * G, dtype=torch.float32, device=x.device)
+    rstd = torch.empty(B * G, dtype=torch.float32, device=x.device)
     if stats is not None and not stats.missing and stats.C == C and stats.rows == B * HW and HW % 32 == 0 and x_bs == 0:
-        _check(L.odise_groupnorm_finalize_seg_f32(stats.ptr, 3 * stats.Ctot, stats.Ctot, _ptr(mean), _ptr(rstd), B, HW, C, G,
-                                                  eps, _stream()), "groupnorm_finalize_seg")
+        lib._launch("odise_groupnorm_finalize_seg_f32", stats.ptr, 3 * stats.Ctot, stats.Ctot, mean, rstd, B, HW, C, G,
+                    eps)
     else:
-        _gn_stats(L, x, ldx, x_bs, mean, rstd, B, HW, C, G, eps)
+        ws = torch.empty(int(lib.load().odise_groupnorm_ws_floats(B, HW, C, G)), dtype=torch.float32, device=x.device)
+        lib._launch("odise_groupnorm_stats_ws_f32", x, ldx, x_bs, ws, mean, rstd, B, HW, C, G, eps)
+    return mean, rstd
 
 
 def group_norm(x, B, HW, gamma, beta, eps, act=ACT_NONE, G=32, want_f32=False, want_planes=True, lo=True, ldx=None,
@@ -39,18 +35,14 @@ def group_norm(x, B, HW, gamma, beta, eps, act=ACT_NONE, G=32, want_f32=False, w
     C = gamma.numel()
     ldx = ldx or x.stride(0)
     dev = x.device
-    mean = torch.empty(B * G, dtype=torch.float32, device=dev)
-    rstd = torch.empty(B * G, dtype=torch.float32, device=dev)
-    L = load()
-    _gn_stats_any(L, x, ldx, x_bs, mean, rstd, B, HW, C, G, eps, stats)
+    mean, rstd = _gn_stats(x, ldx, x_bs, B, HW, C, G, eps, stats)
     if y is None and want_f32:
         y = empty(B * HW, C, dev)
     if y is not None and ldy is None:
         ldy = y.stride(0)
     p = planes if planes is not None else (Planes.empty(B * HW, C, dev, lo=lo) if want_planes else None)
-    _check(L.odise_groupnorm_apply_bs_f32(_ptr(x), ldx, x_bs, _ptr(mean), _ptr(rstd), _ptr(gamma), _ptr(beta), act,
-                                          _ptr(y), ldy or C, y_bs, *lib.pargs(p), o_bs, B, HW, C, G, _stream()),
-           "groupnorm_apply")
+    lib._launch("odise_groupnorm_apply_bs_f32", x, ldx, x_bs, mean, rstd, gamma, beta, act, y, ldy or C, y_bs,
+                *lib.pargs(p), o_bs, B, HW, C, G)
     return y, p
 
 
@@ -59,18 +51,15 @@ def layer_norm(x, gamma, beta, eps=1e-5, res=None, want_f32=False, want_planes=T
     dev = x.device
     y = empty(rows, cols, dev) if want_f32 else None
     p = Planes.empty(rows, cols, dev, lo=lo) if want_planes else None
-    _check(load().odise_layernorm_f32(_ptr(x), x.stride(0), _ptr(res), res.stride(0) if res is not None else 0,
-                                      _ptr(gamma), _ptr(beta), eps, _ptr(y), cols, _ptr(post_add),
-                                      post_add.stride(0) if post_add is not None else 0,
-                                      *lib.pargs(p), rows,
-                                      cols, _stream()), "layernorm")
+    lib._launch("odise_layernorm_f32", x, x.stride(0), res, res.stride(0) if res is not None else 0, gamma, beta, eps,
+                y, cols, post_add, post_add.stride(0) if post_add is not None else 0, *lib.pargs(p), rows, cols)
     return y, p
 
 
 def geglu(x, lo=True):
     rows, c2 = x.shape
     p = Planes.empty(rows, c2 // 2, x.device, lo=lo)
-    _check(load().odise_geglu_f32(_ptr(x), x.stride(0), *lib.pargs(p), rows, c2 // 2, _stream()), "geglu")
+    lib._launch("odise_geglu_f32", x, x.stride(0), *lib.pargs(p), rows, c2 // 2)
     return p
 
 
@@ -78,24 +67,22 @@ def add_split(a, b=None, b_rows=0, want_f32=False, want_planes=True, lo=True):
     rows, cols = a.shape
     y = empty(rows, cols, a.device) if want_f32 else None
     p = Planes.empty(rows, cols, a.device, lo=lo) if want_planes else None
-    _check(load().odise_add_split_f32(_ptr(a), a.stride(0), _ptr(b), b.stride(0) if b is not None else 0, b_rows,
-                                      _ptr(y), cols, *lib.pargs(p), rows, cols, _stream()), "add_split")
+    lib._launch("odise_add_split_f32", a, a.stride(0), b, b.stride(0) if b is not None else 0, b_rows, y, cols,
+                *lib.pargs(p), rows, cols)
     return y, p
 
 
 def act_split(x, act, lo=True):
     rows, cols = x.shape
     p = Planes.empty(rows, cols, x.device, lo=lo)
-    _check(load().odise_act_split_f32(_ptr(x), x.stride(0), act, *lib.pargs(p), rows, cols, _stream()),
-           "act_split")
+    lib._launch("odise_act_split_f32", x, x.stride(0), act, *lib.pargs(p), rows, cols)
     return p
 
 
 def upsample2x_split(x, B, H, W, lo=True):
     C = x.shape[1]
     p = Planes.empty(B * 4 * H * W, C, x.device, lo=lo)
-    _check(load().odise_upsample2x_split_f32(_ptr(x), x.stride(0), *lib.pargs(p), B, H, W, C, _stream()),
-           "upsample2x")
+    lib._launch("odise_upsample2x_split_f32", x, x.stride(0), *lib.pargs(p), B, H, W, C)
     return p
 
 
@@ -105,25 +92,22 @@ def im2col3x3_split(x, B, H, W, stride=1, pad_lo=1, pad_hi=1, lo=True):
     Wo = (W + pad_lo + pad_hi - 3) // stride + 1
     Kpad = (9 * C + 63) // 64 * 64 if lo == lib.Q8 else (9 * C + 7) // 8 * 8
     p = Planes.empty(B * Ho * Wo, Kpad, x.device, lo=lo, ld=Kpad)
-    hi, lo_p, _ = lib.pargs(p)
-    _check(load().odise_im2col3x3_split_f32(_ptr(x), x.stride(0), hi, lo_p, Kpad, B, H, W, C, stride,
-                                            pad_lo, pad_hi, _stream()), "im2col3x3")
+    lib._launch("odise_im2col3x3_split_f32", x, x.stride(0), *lib.pargs(p)[:2], Kpad, B, H, W, C, stride, pad_lo,
+                pad_hi)
     return p, Ho, Wo
 
 
 def copy2d(src, dst, scale=1.0, accumulate=False):
     rows, cols = src.shape
-    _check(load().odise_copy2d_f32(_ptr(src), src.stride(0), _ptr(dst), dst.stride(0), rows, cols, scale,
-                                   1 if accumulate else 0, _stream()), "copy2d")
+    lib._launch("odise_copy2d_f32", src, src.stride(0), dst, dst.stride(0), rows, cols, scale, 1 if accumulate else 0)
 
 
 def resize_nhwc(src, B, Hs, Ws, Hd, Wd, bilinear, dst=None, accumulate=False, src_bs=0, dst_bs=0):
     C = src.shape[1]
     if dst is None:
         dst = empty(B * Hd * Wd, C, src.device)
-    _check(load().odise_resize_nhwc_bs_f32(_ptr(src), src.stride(0), src_bs, _ptr(dst), dst.stride(0), dst_bs, B, Hs,
-                                           Ws, Hd, Wd, C, 1 if bilinear else 0, 1 if accumulate else 0, _stream()),
-           "resize")
+    lib._launch("odise_resize_nhwc_bs_f32", src, src.stride(0), src_bs, dst, dst.stride(0), dst_bs, B, Hs, Ws, Hd, Wd,
+                C, 1 if bilinear else 0, 1 if accumulate else 0)
     return dst
 
 
@@ -131,14 +115,14 @@ def nchw_to_nhwc(x):
     B, C, H, W = x.shape
     x = x.contiguous()
     y = empty(B * H * W, C, x.device)
-    _check(load().odise_nchw_to_nhwc_f32(_ptr(x), _ptr(y), C, B, C, H * W, _stream()), "nchw_to_nhwc")
+    lib._launch("odise_nchw_to_nhwc_f32", x, y, C, B, C, H * W)
     return y
 
 
 def nhwc_to_nchw(x, B, H, W):
     C = x.shape[1]
     y = torch.empty(B, C, H, W, dtype=torch.float32, device=x.device)
-    _check(load().odise_nhwc_to_nchw_f32(_ptr(x), x.stride(0), _ptr(y), B, C, H * W, _stream()), "nhwc_to_nchw")
+    lib._launch("odise_nhwc_to_nchw_f32", x, x.stride(0), y, B, C, H * W)
     return y
 
 
@@ -159,17 +143,14 @@ def attention_tc(q, k, vt, B, heads, d, Tq, Tk, scale, nmma, want_f32=False, wan
     out = empty(B * Tq, C, dev) if want_f32 else None
     p = Planes.empty(B * Tq, C, dev, lo=((nmma == 3) if lo is None else lo)) if want_planes else None
     phi, plo, pld = lib.pargs(p)
-    _check(load().odise_attention_tc(_ptr(q.hi), _ptr(q.lo), q.ld, _ptr(k.hi), _ptr(k.lo), k.ld, _ptr(vt.hi),
-                                     _ptr(vt.lo), vt.ld, vt.rows, _ptr(out), phi,
-                                     plo, pld if p else C, B, heads, d, Tq, Tk, tk_stride or Tk, scale, nmma,
-                                     _ptr(mask_bits), _ptr(row_any), _stream()), "attention_tc")
+    lib._launch("odise_attention_tc", q.hi, q.lo, q.ld, k.hi, k.lo, k.ld, vt.hi, vt.lo, vt.ld, vt.rows, out, phi, plo,
+                pld if p else C, B, heads, d, Tq, Tk, tk_stride or Tk, scale, nmma, mask_bits, row_any)
     return out, p
 
 
 def softmax_split(x, rows, cols, cols_pad, scale, lo=True):
     p = Planes.empty(rows, cols_pad, x.device, lo=lo, ld=cols_pad)
-    _check(load().odise_softmax_split_f32(_ptr(x), x.stride(0), *lib.pargs(p), rows, cols, cols_pad,
-                                          scale, _stream()), "softmax_split")
+    lib._launch("odise_softmax_split_f32", x, x.stride(0), *lib.pargs(p), rows, cols, cols_pad, scale)
     return p
 
 
@@ -195,9 +176,8 @@ def msda_fused(value, spatial_shapes, level_start, ref, offs, logits, N, S, M, D
     dev = value.device
     out = empty(N * Lq, M * D, dev) if want_f32 else None
     p = Planes.empty(N * Lq, M * D, dev, lo=lo)
-    _check(load().odise_msda_fused_f32(_ptr(value), _ptr(spatial_shapes), _ptr(level_start), _ptr(ref), _ptr(offs),
-                                       _ptr(logits), _ptr(out), *lib.pargs(p)[:2], N, S, M, D, L, Lq, P,
-                                       _stream()), "msda_fused")
+    lib._launch("odise_msda_fused_f32", value, spatial_shapes, level_start, ref, offs, logits, out, *lib.pargs(p)[:2],
+                N, S, M, D, L, Lq, P)
     return out, p
 
 
@@ -205,19 +185,17 @@ def attn_mask_bits(mask_logits, B, Q, Hm, Wm, Hl, Wl):
     dev = mask_logits.device
     bits = torch.empty(B * Q * ((Hl * Wl + 31) // 32), dtype=torch.int32, device=dev)
     row_any = torch.empty(B * Q, dtype=torch.int32, device=dev)
-    _check(load().odise_attn_mask_bits_f32(_ptr(mask_logits), _ptr(bits), _ptr(row_any), B, Q, Hm, Wm, Hl, Wl,
-                                           _stream()), "attn_mask_bits")
+    lib._launch("odise_attn_mask_bits_f32", mask_logits, bits, row_any, B, Q, Hm, Wm, Hl, Wl)
     return bits, row_any
 
 
 def mha_d32(q, ldq, k, v, ldkv, B, Tq, Tk, heads, scale, bits=None, row_any=None, lo=True):
     """q/k/v fp32 device tensors (any views whose data_ptr is the first element); returns Planes [B*Tq, heads*32]."""
     p = Planes.empty(B * Tq, heads * 32, q.device, lo=lo)
-    L = load()
-    nws = int(L.odise_mha_d32_ws_floats(B, Tq, Tk, heads))
+    nws = int(lib.load().odise_mha_d32_ws_floats(B, Tq, Tk, heads))
     ws = torch.empty(nws, dtype=torch.float32, device=q.device) if nws else None
-    _check(L.odise_mha_d32_ws_f32(_ptr(q), ldq, _ptr(k), _ptr(v), ldkv, _ptr(bits), _ptr(row_any), None, *lib.pargs(p),
-                                  B, Tq, Tk, heads, scale, _ptr(ws), _stream()), "mha_d32")
+    lib._launch("odise_mha_d32_ws_f32", q, ldq, k, v, ldkv, bits, row_any, None, *lib.pargs(p), B, Tq, Tk, heads, scale,
+                ws)
     return p
 
 
@@ -225,85 +203,78 @@ def mask_binarize(logits, B, Q, HW):
     dev = logits.device
     binp = torch.empty(B * Q * HW, dtype=torch.bfloat16, device=dev)
     counts = torch.empty(B * Q, dtype=torch.float32, device=dev)
-    _check(load().odise_mask_binarize_f32(_ptr(logits), _ptr(binp), HW, _ptr(counts), B, Q, HW, _stream()),
-           "mask_binarize")
+    lib._launch("odise_mask_binarize_f32", logits, binp, HW, counts, B, Q, HW)
     return binp, counts
 
 
 def pool_normalize(sums, counts, B, Q, C):
     out = empty(B * Q, C, sums.device)
-    _check(load().odise_pool_normalize_f32(_ptr(sums), _ptr(counts), _ptr(out), B, Q, C, _stream()), "pool_normalize")
+    lib._launch("odise_pool_normalize_f32", sums, counts, out, B, Q, C)
     return out
 
 
 def l2_normalize_split(x, lo=True):
     rows, cols = x.shape
     p = Planes.empty(rows, cols, x.device, lo=lo)
-    _check(load().odise_l2_normalize_split_f32(_ptr(x), x.stride(0), *lib.pargs(p), rows, cols,
-                                               _stream()), "l2_normalize")
+    lib._launch("odise_l2_normalize_split_f32", x, x.stride(0), *lib.pargs(p), rows, cols)
     return p
 
 
 def class_max(sims, group_start, null_sim, rows, n_classes):
     out = empty(rows, n_classes + 1, sims.device)
-    _check(load().odise_class_max_f32(_ptr(sims), sims.stride(0), _ptr(group_start), _ptr(null_sim), _ptr(out), rows,
-                                      n_classes, _stream()), "class_max")
+    lib._launch("odise_class_max_f32", sims, sims.stride(0), group_start, null_sim, out, rows, n_classes)
     return out
 
 
 def group_norm_res(x, B, HW, gamma, beta, eps, res, act, y, accumulate, G=32, stats=None):
     """y (+)= act(gn(x) + res); x, res, y dense [B*HW, C] fp32."""
     C = gamma.numel()
-    dev = x.device
-    mean = torch.empty(B * G, dtype=torch.float32, device=dev)
-    rstd = torch.empty(B * G, dtype=torch.float32, device=dev)
-    L = load()
-    _gn_stats_any(L, x, x.stride(0), 0, mean, rstd, B, HW, C, G, eps, stats)
-    _check(L.odise_groupnorm_apply_res_f32(_ptr(x), x.stride(0), _ptr(mean), _ptr(rstd), _ptr(gamma), _ptr(beta),
-                                           _ptr(res), res.stride(0) if res is not None else 0, act, _ptr(y),
-                                           y.stride(0), 1 if accumulate else 0, None, None, 0, B, HW, C, G, _stream()),
-           "groupnorm_apply_res")
+    mean, rstd = _gn_stats(x, x.stride(0), 0, B, HW, C, G, eps, stats)
+    lib._launch("odise_groupnorm_apply_res_f32", x, x.stride(0), mean, rstd, gamma, beta, res,
+                res.stride(0) if res is not None else 0, act, y, y.stride(0), 1 if accumulate else 0, None, None, 0,
+                B, HW, C, G)
     return y
 
 
 def bcast_fma(a0, ta, p, B, T, C):
     out = torch.empty(B * T, C, dtype=torch.float32, device=p.device)
-    _check(load().odise_bcast_fma_f32(_ptr(a0), _ptr(ta), _ptr(p), _ptr(out), B, T, C, _stream()), "bcast_fma")
+    lib._launch("odise_bcast_fma_f32", a0, ta, p, out, B, T, C)
     return out
 
 
 def rowscale(y, s):
     rows, cols = y.shape
-    _check(load().odise_rowscale_f32(_ptr(y), y.stride(0), _ptr(s), rows, cols, _stream()), "rowscale")
+    lib._launch("odise_rowscale_f32", y, y.stride(0), s, rows, cols)
     return y
+
+
+def _is_u8_image(img, what):
+    """1 for a uint8 image (0..255), 0 for a float32 one (in [0, 1]); OdiseError for any other dtype"""
+    if img.dtype not in (torch.uint8, torch.float32):
+        raise lib.OdiseError(f"{what}: uint8 or float32 image expected")
+    return int(img.dtype == torch.uint8)
 
 
 def image_crops(img, boxes_dev, n_crops, H, W, ch, cw):
     """uint8 [N,3,H,W] (0..255) or float32 [N,3,H,W] in [0,1] -> normalised NHWC crops [n_crops*ch*cw, 3]."""
+    fn = "odise_image_crops_u8_f32" if _is_u8_image(img, "image_crops") else "odise_image_crops_f32"
     out = torch.empty(n_crops * ch * cw, 3, dtype=torch.float32, device=img.device)
-    fn = load().odise_image_crops_u8_f32 if img.dtype == torch.uint8 else load().odise_image_crops_f32
-    if img.dtype not in (torch.uint8, torch.float32):
-        raise lib.OdiseError("image_crops: uint8 or float32 image expected")
-    _check(fn(_ptr(img), _ptr(out), _ptr(boxes_dev), n_crops, H, W, ch, cw, _stream()), "image_crops")
+    lib._launch(fn, img, out, boxes_dev, n_crops, H, W, ch, cw)
     return out
 
 
 def clip_preprocess(img, boxes_dev, n_crops, H, W, ch, cw, S=336):
+    u8 = _is_u8_image(img, "clip_preprocess")
     out = torch.empty(n_crops * S * S, 3, dtype=torch.float32, device=img.device)
-    if img.dtype not in (torch.uint8, torch.float32):
-        raise lib.OdiseError("clip_preprocess: uint8 or float32 image expected")
-    _check(load().odise_clip_preprocess(_ptr(img), 1 if img.dtype == torch.uint8 else 0, _ptr(out), _ptr(boxes_dev),
-                                        n_crops, H, W, ch, cw, S, _stream()), "clip_preprocess")
+    lib._launch("odise_clip_preprocess", img, u8, out, boxes_dev, n_crops, H, W, ch, cw, S)
     return out
 
 
 def crop_resize_bicubic(img, boxes_dev, n_crops, H, W, ch, cw, S=512):
     """T.Resize((S, S), BICUBIC) of every crop -> float image batch NCHW [n_crops, 3, S, S] (feature_extractor.py:73-76)."""
-    if img.dtype not in (torch.uint8, torch.float32):
-        raise lib.OdiseError("crop_resize_bicubic: uint8 or float32 image expected")
+    u8 = _is_u8_image(img, "crop_resize_bicubic")
     out = torch.empty(n_crops, 3, S, S, dtype=torch.float32, device=img.device)
-    _check(load().odise_crop_resize_bicubic(_ptr(img), 1 if img.dtype == torch.uint8 else 0, _ptr(out), _ptr(boxes_dev),
-                                            n_crops, H, W, ch, cw, S, _stream()), "crop_resize_bicubic")
+    lib._launch("odise_crop_resize_bicubic", img, u8, out, boxes_dev, n_crops, H, W, ch, cw, S)
     return out
 
 
@@ -311,18 +282,15 @@ def patchify_split(x, B, S, P, lo=True):
     Kpad = (3 * P * P + 63) // 64 * 64 if lo == lib.Q8 else (3 * P * P + 7) // 8 * 8
     G = S // P
     p = Planes.empty(B * G * G, Kpad, x.device, lo=lo, ld=Kpad)
-    hi, lo_p, _ = lib.pargs(p)
-    _check(load().odise_patchify_split_f32(_ptr(x), hi, lo_p, B, S, P, Kpad, _stream()), "patchify")
+    lib._launch("odise_patchify_split_f32", x, *lib.pargs(p)[:2], B, S, P, Kpad)
     return p
 
 
 def maskclip_preprocess(img, N, H, W, S=336):
     """whole image [N,3,H,W] (u8 0..255 / f32 in [0,1]) -> bilinear S x S + CLIP normalisation, NHWC [N*S*S, 3]."""
-    if img.dtype not in (torch.uint8, torch.float32):
-        raise lib.OdiseError("maskclip_preprocess: uint8 or float32 image expected")
+    u8 = _is_u8_image(img, "maskclip_preprocess")
     out = torch.empty(N * S * S, 3, dtype=torch.float32, device=img.device)
-    _check(load().odise_maskclip_preprocess(_ptr(img), 1 if img.dtype == torch.uint8 else 0, _ptr(out), N, H, W, S,
-                                            _stream()), "maskclip_preprocess")
+    lib._launch("odise_maskclip_preprocess", img, u8, out, N, H, W, S)
     return out
 
 
@@ -332,16 +300,15 @@ def maskclip_bits(mask_logits, B, Q, hm, wm, S, P, Tq, row0):
     words = (G * G + 1 + 31) // 32
     bits = torch.zeros(B, Tq, words, dtype=torch.int32, device=mask_logits.device)
     row_any = torch.empty(B, Tq, dtype=torch.int32, device=mask_logits.device)
-    _check(load().odise_maskclip_bits_f32(_ptr(mask_logits), _ptr(bits), _ptr(row_any), B, Q, hm, wm, S, P, Tq, row0,
-                                          _stream()), "maskclip_bits")
+    lib._launch("odise_maskclip_bits_f32", mask_logits, bits, row_any, B, Q, hm, wm, S, P, Tq, row0)
     return bits, row_any
 
 
 def open_vocab_merge(cat_logits, clip_logits, ld_clip, overlap_u8, alpha, beta, rows, K, want_open=False):
     out = torch.empty(rows, K + 1, dtype=torch.float32, device=cat_logits.device)
     op = torch.empty(rows, K, dtype=torch.float32, device=cat_logits.device) if want_open else None
-    _check(load().odise_open_vocab_merge_f32(_ptr(cat_logits), _ptr(clip_logits), ld_clip, _ptr(overlap_u8), alpha, beta,
-                                             _ptr(out), _ptr(op), rows, K, _stream()), "open_vocab_merge")
+    lib._launch("odise_open_vocab_merge_f32", cat_logits, clip_logits, ld_clip, overlap_u8, alpha, beta, out, op, rows,
+                K)
     return out, op
 
 
@@ -349,6 +316,6 @@ def gather_rows(src, idx, add=None, add_period=1):
     """out[i] = src[idx[i]] (+ add[i % add_period]); src fp32 [n, cols], idx int32 [rows]."""
     rows, cols = idx.numel(), src.shape[1]
     out = empty(rows, cols, src.device)
-    _check(load().odise_gather_rows_f32(_ptr(src), src.stride(0), _ptr(idx), _ptr(add), add.stride(0) if add is not None else 0,
-                                        add_period, _ptr(out), cols, rows, cols, _stream()), "gather_rows")
+    lib._launch("odise_gather_rows_f32", src, src.stride(0), idx, add, add.stride(0) if add is not None else 0,
+                add_period, out, cols, rows, cols)
     return out

@@ -6,8 +6,8 @@ sem_seg_postprocess_before_inference=True in every ODISE config) is folded into 
 import ctypes
 import torch
 
-from . import lib, ops
-from .lib import Planes, _check, _ptr, _stream, load
+from . import lib
+from .lib import Planes
 
 
 class PostProcessor:
@@ -35,7 +35,7 @@ class PostProcessor:
         B, Q, K1 = pred_logits.shape
         assert K1 == self.K + 1
         hs, ws = pred_masks.shape[-2:]
-        dev, L = self.dev, load()
+        dev, L = self.dev, lib.load()
         geom = None
         if padded_size is not None or image_size is not None:
             ph, pw = padded_size if padded_size is not None else (H, W)
@@ -49,8 +49,7 @@ class PostProcessor:
         keep = torch.empty(B * Q, dtype=torch.int32, device=dev)
         cl = pred_logits.contiguous()
         probs = torch.empty(B * Q, K1, dtype=torch.float32, device=dev) if instance else None
-        _check(L.odise_query_scores_f32(_ptr(cl), _ptr(probs), _ptr(probs_t), _ptr(scores), _ptr(labels), _ptr(keep), B, Q, Qp,
-                                        K1, self.obj_thr, _stream()), "query_scores")
+        lib._launch("odise_query_scores_f32", cl, probs, probs_t, scores, labels, keep, B, Q, Qp, K1, self.obj_thr)
         out = {}
         pm = pred_masks.contiguous()
         # ONE resampling pass over the mask logits feeds all requested heads (odise_postprocess_fused_f32)
@@ -70,14 +69,12 @@ class PostProcessor:
             qm = torch.empty(B, Q, H, W, dtype=torch.uint8, device=dev) if instance_masks else None
             iws = torch.empty(int(L.odise_postprocess_fused_ws_bytes(B, Q, H, W)), dtype=torch.uint8, device=dev)
         if semantic or panoptic or instance:
-          _check(L.odise_postprocess_fused_f32(
-              _ptr(pm), _ptr(sig.hi) if sig else None, _ptr(sig.lo) if sig else None, Qp, _ptr(scores), _ptr(labels),
-              _ptr(keep), _ptr(self.is_thing), _ptr(pan), _ptr(seg_info), _ptr(nseg), _ptr(pws), self.ov_thr, _ptr(probs),
-              _ptr(i_sc), _ptr(i_cl), _ptr(i_q), _ptr(i_ok), _ptr(qm), _ptr(iws), topk, 1 if panoptic_on else 0, B, Q, self.K,
-              hs, ws, H, W, geom, _stream()), "postprocess_fused")
+            lib._launch("odise_postprocess_fused_f32", pm, sig.hi if sig else None, sig.lo if sig else None, Qp, scores,
+                        labels, keep, self.is_thing, pan, seg_info, nseg, pws, self.ov_thr, probs, i_sc, i_cl, i_q, i_ok,
+                        qm, iws, topk, 1 if panoptic_on else 0, B, Q, self.K, hs, ws, H, W, geom)
         if semantic:
             # sem[b] = P_b^T [K, Q] @ sig_b^T [Q, HW]: swapped-operand GEMM writes the reference's [K, H, W] layout
-            ptp = ops.split(probs_t, lo=self.lo)
+            ptp = lib.split(probs_t, lo=self.lo)
             sem = torch.empty(B, self.K, H * W, dtype=torch.float32, device=dev)
             lib.gemm(ptp, sig, M=self.K, N=H * W, K=Qp, nmma=self.nmma, batch=B, a_bs=self.K * ptp.ld, b_bs=H * W * sig.ld,
                      out=sem, ld_out=H * W, out_bs=self.K * H * W)

@@ -171,7 +171,7 @@ class UNetEngine:
                                 want_f32=not imp, want_planes=imp, stats=hs)
         if cin != cout:
             skip = ops.empty(M, cout, self.dev)
-            self._gemm(ops.split(x, lo=self.lo), q + "skip", q + "skip.b", out=skip)
+            self._gemm(lib.split(x, lo=self.lo), q + "skip", q + "skip.b", out=skip)
         else:
             skip = x
         if imp:
@@ -254,7 +254,7 @@ class UNetEngine:
             y1, n1 = ops.layer_norm(h, self.F[t + "norm1.g"], self.F[t + "norm1.b"], lo=self.lo, want_f32=True)
             kvp = torch.zeros(B, TkS * ch, dtype=torch.float32, device=self.dev)
             ops.copy2d(y1.view(B, T * ch), kvp[:, :T * ch])
-            o1 = self._attention(t, "attn1", n1, ops.split(kvp.view(B * TkS, ch), lo=self.lo), B, T, T, ch, TkS=TkS)
+            o1 = self._attention(t, "attn1", n1, lib.split(kvp.view(B * TkS, ch), lo=self.lo), B, T, T, ch, TkS=TkS)
         h2 = ops.empty(M, ch, self.dev)
         self._gemm(o1, t + "attn1.out", t + "attn1.out.b", residual=h, out=h2)
         _, n2 = ops.layer_norm(h2, self.F[t + "norm2.g"], self.F[t + "norm2.b"], lo=self.lo)
@@ -286,7 +286,7 @@ class UNetEngine:
         cpad = torch.zeros(B, CTX_TS, context.shape[1], dtype=torch.float32, device=dev)
         nc = CTX_T * context.shape[1]
         ops.copy2d(context.view(B, nc), cpad.view(B, CTX_TS * context.shape[1])[:, :nc])
-        ctx = ops.split(cpad.view(B * CTX_TS, -1), lo=self.lo)
+        ctx = lib.split(cpad.view(B * CTX_TS, -1), lo=self.lo)
 
         # spatial size / channels of every down-path output (= skip), to lay out the concat buffers
         sizes = []
@@ -320,7 +320,7 @@ class UNetEngine:
                 # ldm Downsample = conv3x3 stride 2 pad 1: strided implicit GEMM (TMA element strides), no im2col
                 cdim = layers[0][1]
                 if lib.conv_ok(ch_ // 2, cw_ // 2):
-                    self._gemm(ops.split(cur, lo=self.lo), q + "0.conv", q + "0.conv.b", M=B * (ch_ // 2) * (cw_ // 2),
+                    self._gemm(lib.split(cur, lo=self.lo), q + "0.conv", q + "0.conv.b", M=B * (ch_ // 2) * (cw_ // 2),
                                N=cdim, conv=(cdim, ch_, cw_), conv_mode=1, out=dst, gn=dst_s)
                 else:
                     self._gemm(ops.im2col3x3_split(cur, B, ch_, cw_, stride=2, lo=self.lo)[0], q + "0.conv", q + "0.conv.b",

@@ -107,7 +107,7 @@ class VAEEngine:
         _, a2 = self._gn(h, B, H * W, n + "n2", ACT_SILU, stats=hs)
         if cin != cout:
             skip = ops.empty(M, cout, self.dev)
-            self._gemm(ops.split(x, lo=self.lo), n + "sc", out=skip)
+            self._gemm(lib.split(x, lo=self.lo), n + "sc", out=skip)
         else:
             skip = x
         out = ops.empty(M, cout, self.dev)
@@ -155,7 +155,7 @@ class VAEEngine:
                 # strided implicit GEMM: conv_mode 2 = stride 2 with zero padding on the high side only
                 d = ops.empty(B * (ch // 2) * (cw // 2), cout, self.dev)
                 hs = lib.GnStats(B * (ch // 2) * (cw // 2), cout, self.dev)
-                self._gemm(ops.split(h, lo=self.lo), f"e.d{lvl}.down", M=B * (ch // 2) * (cw // 2), N=cout,
+                self._gemm(lib.split(h, lo=self.lo), f"e.d{lvl}.down", M=B * (ch // 2) * (cw // 2), N=cout,
                            conv=(cout, ch, cw), conv_mode=2, out=d, gn=hs)
                 ch, cw = ch // 2, cw // 2
                 h = d
@@ -181,7 +181,7 @@ class VAEEngine:
         z8 = torch.zeros(B * h * w, 8, dtype=torch.float32, device=self.dev)
         ops.copy2d(z, z8[:, :4])
         pq = ops.empty(B * h * w, 4, self.dev)
-        self._gemm(ops.split(z8, lo=self.lo), "post_quant", out=pq)
+        self._gemm(lib.split(z8, lo=self.lo), "post_quant", out=pq)
         cols, _, _ = ops.im2col3x3_split(pq, B, h, w, lo=self.lo)
         x = ops.empty(B * h * w, 512, self.dev)
         xs = lib.GnStats(B * h * w, 512, self.dev)

@@ -3,6 +3,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from odise_b200 import lib
+
 pytestmark = pytest.mark.gpu
 
 
@@ -10,16 +12,9 @@ def _rel(a, b):
     return ((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-30)).item()
 
 
-def _call(name, *args):
-    from odise_b200 import lib
-    rc = getattr(lib.load(), name)(*args, torch.cuda.current_stream().cuda_stream)
-    assert rc == 0, (name, rc)
-
-
 @pytest.mark.parametrize("shape", [(2, 64 * 64, 320, 32), (3, 16 * 16, 1920, 32), (1, 8 * 8, 2560, 32), (2, 100, 256, 32)])
 @pytest.mark.parametrize("act", [0, 2, 1])
 def test_groupnorm(cuda, shape, act):
-    from odise_b200 import lib
     B, HW, C, G = shape
     g = torch.Generator().manual_seed(C)
     x = (torch.randn(B, HW, C, generator=g) * 2 + 0.7).to(cuda)
@@ -27,9 +22,8 @@ def test_groupnorm(cuda, shape, act):
     mean, rstd = torch.empty(B * G, device=cuda), torch.empty(B * G, device=cuda)
     y = torch.empty_like(x)
     yp = lib.Planes.empty(B * HW, C, cuda)
-    _call("odise_groupnorm_stats_f32", x.data_ptr(), C, mean.data_ptr(), rstd.data_ptr(), B, HW, C, G, 1e-5)
-    _call("odise_groupnorm_apply_f32", x.data_ptr(), C, mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(),
-          beta.data_ptr(), act, y.data_ptr(), C, yp.hi.data_ptr(), yp.lo.data_ptr(), yp.ld, B, HW, C, G)
+    lib._launch("odise_groupnorm_stats_f32", x, C, mean, rstd, B, HW, C, G, 1e-5)
+    lib._launch("odise_groupnorm_apply_f32", x, C, mean, rstd, gamma, beta, act, y, C, yp.hi, yp.lo, yp.ld, B, HW, C, G)
     ref = F.group_norm(x.double().transpose(1, 2), G, gamma.double(), beta.double(), 1e-5).transpose(1, 2)
     ref = [lambda t: t, F.relu, F.silu][act](ref)
     assert _rel(y, ref) < 2e-6
@@ -38,7 +32,6 @@ def test_groupnorm(cuda, shape, act):
 
 @pytest.mark.parametrize("cols", [256, 320, 640, 1280, 2048])
 def test_layernorm(cuda, cols):
-    from odise_b200 import lib
     rows = 333
     g = torch.Generator().manual_seed(cols)
     x, res = torch.randn(rows, cols, generator=g).to(cuda), torch.randn(rows, cols, generator=g).to(cuda)
@@ -46,36 +39,34 @@ def test_layernorm(cuda, cols):
     gamma, beta = torch.randn(cols, generator=g).to(cuda), torch.randn(cols, generator=g).to(cuda)
     y = torch.empty_like(x)
     yp = lib.Planes.empty(rows, cols, cuda)
-    _call("odise_layernorm_f32", x.data_ptr(), cols, res.data_ptr(), cols, gamma.data_ptr(), beta.data_ptr(), 1e-5,
-          y.data_ptr(), cols, pa.data_ptr(), cols, yp.hi.data_ptr(), yp.lo.data_ptr(), yp.ld, rows, cols)
+    lib._launch("odise_layernorm_f32", x, cols, res, cols, gamma, beta, 1e-5, y, cols, pa, cols, yp.hi, yp.lo, yp.ld,
+                rows, cols)
     ref = F.layer_norm((x + res).double(), (cols,), gamma.double(), beta.double(), 1e-5)
     assert _rel(y, ref) < 2e-6
     assert _rel(yp.float(), ref + pa.double()) < 2e-5
 
 
 def test_geglu_add_upsample_copy(cuda):
-    from odise_b200 import lib
     g = torch.Generator().manual_seed(1)
     x = torch.randn(77, 2 * 640, generator=g).to(cuda)
     p = lib.Planes.empty(77, 640, cuda)
-    _call("odise_geglu_f32", x.data_ptr(), 1280, p.hi.data_ptr(), p.lo.data_ptr(), p.ld, 77, 640)
+    lib._launch("odise_geglu_f32", x, 1280, p.hi, p.lo, p.ld, 77, 640)
     ref = x[:, :640].double() * F.gelu(x[:, 640:].double())
     assert _rel(p.float(), ref) < 2e-5
     a, b = torch.randn(200, 256, generator=g).to(cuda), torch.randn(100, 256, generator=g).to(cuda)
     y = torch.empty_like(a)
     p = lib.Planes.empty(200, 256, cuda)
-    _call("odise_add_split_f32", a.data_ptr(), 256, b.data_ptr(), 256, 100, y.data_ptr(), 256, p.hi.data_ptr(),
-          p.lo.data_ptr(), p.ld, 200, 256)
+    lib._launch("odise_add_split_f32", a, 256, b, 256, 100, y, 256, p.hi, p.lo, p.ld, 200, 256)
     assert torch.equal(y, a + b.repeat(2, 1))
     assert _rel(p.float(), y) < 2e-5
     u = torch.randn(2, 5, 7, 64, generator=g).to(cuda)
     p = lib.Planes.empty(2 * 10 * 14, 64, cuda)
-    _call("odise_upsample2x_split_f32", u.data_ptr(), 64, p.hi.data_ptr(), p.lo.data_ptr(), p.ld, 2, 5, 7, 64)
+    lib._launch("odise_upsample2x_split_f32", u, 64, p.hi, p.lo, p.ld, 2, 5, 7, 64)
     ref = F.interpolate(u.permute(0, 3, 1, 2), scale_factor=2, mode="nearest").permute(0, 2, 3, 1).reshape(-1, 64)
     assert _rel(p.float(), ref) < 2e-5
     dst = torch.ones(50, 128, device=cuda)
     src = torch.randn(50, 64, generator=g).to(cuda)
-    _call("odise_copy2d_f32", src.data_ptr(), 64, dst[:, 32:].data_ptr(), 128, 50, 64, 0.5, 1)
+    lib._launch("odise_copy2d_f32", src, 64, dst[:, 32:], 128, 50, 64, 0.5, 1)
     assert torch.allclose(dst[:, 32:96], 1 + 0.5 * src) and dst[:, :32].eq(1).all() and dst[:, 96:].eq(1).all()
 
 
@@ -97,7 +88,7 @@ def test_resize(cuda, cfg):
     ref = ref.permute(0, 2, 3, 1)
     if len(cfg) == 7:
         y = torch.zeros(B, Hd, Wd, C, device=cuda)
-        _call("odise_resize_nhwc_f32", x.data_ptr(), C, y.data_ptr(), C, B, Hs, Ws, Hd, Wd, C, bil, 0)
+        lib._launch("odise_resize_nhwc_f32", x, C, y, C, B, Hs, Ws, Hd, Wd, C, bil, 0)
     else:
         from odise_b200 import ops
         r0 = cfg[7]
@@ -114,7 +105,6 @@ def test_resize(cuda, cfg):
 
 @pytest.mark.parametrize("cfg", [(2, 9, 9, 4, 1, 1, 1), (1, 16, 16, 320, 2, 1, 1), (1, 16, 16, 128, 2, 0, 1), (2, 8, 8, 3, 1, 1, 1)])
 def test_im2col(cuda, cfg):
-    from odise_b200 import lib
     B, H, W, C, stride, plo, phi = cfg
     g = torch.Generator().manual_seed(C)
     x = torch.randn(B, C, H, W, generator=g).to(cuda)
@@ -125,8 +115,7 @@ def test_im2col(cuda, cfg):
     Kpad = (9 * C + 7) // 8 * 8
     xh = x.permute(0, 2, 3, 1).contiguous()
     cols = lib.Planes.empty(B * Ho * Wo, Kpad, cuda, ld=Kpad)
-    _call("odise_im2col3x3_split_f32", xh.data_ptr(), C, cols.hi.data_ptr(), cols.lo.data_ptr(), Kpad, B, H, W, C,
-          stride, plo, phi)
+    lib._launch("odise_im2col3x3_split_f32", xh, C, cols.hi, cols.lo, Kpad, B, H, W, C, stride, plo, phi)
     wm = torch.zeros(24, Kpad, device=cuda)
     wm[:, :9 * C] = w.permute(0, 2, 3, 1).reshape(24, 9 * C)
     out = torch.empty(B * Ho * Wo, 24, device=cuda)
@@ -137,19 +126,18 @@ def test_im2col(cuda, cfg):
 def test_transposes(cuda):
     x = torch.randn(2, 37, 50, device=cuda)       # NCHW [B, C, HW]
     y = torch.empty(2, 50, 40, device=cuda)
-    _call("odise_nchw_to_nhwc_f32", x.data_ptr(), y.data_ptr(), 40, 2, 37, 50)
+    lib._launch("odise_nchw_to_nhwc_f32", x, y, 40, 2, 37, 50)
     assert torch.equal(y[:, :, :37], x.transpose(1, 2))
     z = torch.empty(2, 37, 50, device=cuda)
-    _call("odise_nhwc_to_nchw_f32", y.data_ptr(), 40, z.data_ptr(), 2, 37, 50)
+    lib._launch("odise_nhwc_to_nchw_f32", y, 40, z, 2, 37, 50)
     assert torch.equal(z, x)
 
 
 def test_clip_tail(cuda):
-    from odise_b200 import lib
     g = torch.Generator().manual_seed(2)
     x = torch.randn(100, 256, generator=g).to(cuda)
     p = lib.Planes.empty(100, 256, cuda)
-    _call("odise_l2_normalize_split_f32", x.data_ptr(), 256, p.hi.data_ptr(), p.lo.data_ptr(), p.ld, 100, 256)
+    lib._launch("odise_l2_normalize_split_f32", x, 256, p.hi, p.lo, p.ld, 100, 256)
     assert _rel(p.float(), F.normalize(x.double(), dim=-1)) < 2e-5
     sizes = torch.randint(1, 5, (20,), generator=g)
     gs = torch.cat([torch.zeros(1, dtype=torch.long), sizes.cumsum(0)]).int().to(cuda)
@@ -157,7 +145,7 @@ def test_clip_tail(cuda):
     sims = torch.randn(100, Kp, generator=g).to(cuda)
     null = torch.randn(100, generator=g).to(cuda)
     out = torch.empty(100, 21, device=cuda)
-    _call("odise_class_max_f32", sims.data_ptr(), Kp, gs.data_ptr(), null.data_ptr(), out.data_ptr(), 100, 20)
+    lib._launch("odise_class_max_f32", sims, Kp, gs, null, out, 100, 20)
     ref = torch.stack([sims[:, gs[i]:gs[i + 1]].max(-1).values for i in range(20)] + [null], -1)
     assert torch.equal(out, ref)
 
@@ -167,12 +155,12 @@ def test_mask_pool_helpers(cuda):
     logits = torch.randn(2, 10, 64 * 64, generator=g).to(cuda)
     binm = torch.empty(2, 10, 64 * 64, dtype=torch.bfloat16, device=cuda)
     cnt = torch.empty(2, 10, device=cuda)
-    _call("odise_mask_binarize_f32", logits.data_ptr(), binm.data_ptr(), 64 * 64, cnt.data_ptr(), 2, 10, 64 * 64)
+    lib._launch("odise_mask_binarize_f32", logits, binm, 64 * 64, cnt, 2, 10, 64 * 64)
     ref = (logits.sigmoid() > 0.5).float()
     assert torch.equal(binm.float(), ref) and torch.equal(cnt, ref.sum(-1))
     sums = torch.randn(2, 10, 256, generator=g).to(cuda)
     pooled = torch.empty_like(sums)
-    _call("odise_pool_normalize_f32", sums.data_ptr(), cnt.data_ptr(), pooled.data_ptr(), 2, 10, 256)
+    lib._launch("odise_pool_normalize_f32", sums, cnt, pooled, 2, 10, 256)
     assert torch.allclose(pooled, sums / (cnt[..., None] + 1e-8), rtol=1e-6)
 
 
@@ -222,15 +210,14 @@ def test_mha_d32(cuda, cfg):
         ml[0, 3] = -5.0          # a fully masked row -> must attend everywhere
         bits = torch.empty(B, Tq, (Tk + 31) // 32, dtype=torch.int32, device=cuda)
         rowany = torch.empty(B, Tq, dtype=torch.int32, device=cuda)
-        _call("odise_attn_mask_bits_f32", ml.data_ptr(), bits.data_ptr(), rowany.data_ptr(), B, Tq, Hm, Wm, Hl, Wl)
+        lib._launch("odise_attn_mask_bits_f32", ml, bits, rowany, B, Tq, Hm, Wm, Hl, Wl)
         check_mask_bits(bits, rowany, ml, Hl, Wl)
         am = F.interpolate(ml, size=(Hl, Wl), mode="bilinear", align_corners=False).sigmoid().flatten(2) < 0.5
         am[torch.where(am.sum(-1) == am.shape[-1])] = False
         assert rowany[0, 3].item() == 0
         bias = torch.zeros(B, 1, Tq, Tk, device=cuda, dtype=torch.float64).masked_fill(am[:, None], float("-inf"))
-    _call("odise_mha_d32_f32", q.data_ptr(), heads * d, k.data_ptr(), v.data_ptr(), heads * d,
-          None if bits is None else bits.data_ptr(), None if rowany is None else rowany.data_ptr(), out.data_ptr(),
-          None, None, heads * d, B, Tq, Tk, heads, scale)
+    lib._launch("odise_mha_d32_f32", q, heads * d, k, v, heads * d, bits, rowany, out, None, None, heads * d, B, Tq, Tk,
+                heads, scale)
     qh = q.double().view(B, Tq, heads, d).transpose(1, 2)
     kh = k.double().view(B, Tk, heads, d).transpose(1, 2)
     vh = v.double().view(B, Tk, heads, d).transpose(1, 2)

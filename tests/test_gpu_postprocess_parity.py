@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import postprocess_ref as pr
+from odise_b200 import lib
 
 pytestmark = pytest.mark.gpu
 
@@ -33,14 +34,7 @@ def _is_thing(K, things, dev):
     return t.to(dev)
 
 
-def _call(name, *args):
-    from odise_b200 import lib
-    rc = getattr(lib.load(), name)(*args, torch.cuda.current_stream().cuda_stream)
-    assert rc == 0, (name, rc)
-
-
 def _geom(geom):
-    from odise_b200 import lib
     return None if geom is None else ctypes.byref(lib.PostprocessGeom(*geom))
 
 
@@ -51,8 +45,8 @@ def _query_scores(cls, thr=0.0):
     probs = torch.empty(B * Q, K1, device=dev)
     scores = torch.empty(B * Q, device=dev)
     labels, keep = (torch.empty(B * Q, dtype=torch.int32, device=dev) for _ in range(2))
-    _call("odise_query_scores_f32", cls.contiguous().data_ptr(), probs.data_ptr(), None, scores.data_ptr(),
-          labels.data_ptr(), keep.data_ptr(), B, Q, (Q + 7) // 8 * 8, K1, thr)
+    lib._launch("odise_query_scores_f32", cls.contiguous(), probs, None, scores, labels, keep, B, Q, (Q + 7) // 8 * 8,
+                K1, thr)
     return probs, scores, labels, keep
 
 
@@ -395,24 +389,21 @@ def test_standalone_entry_points(cuda, record, geom):
     it = _is_thing(K, things, cuda)
     hi, lo = (torch.zeros(B * H * W, Qp, dtype=torch.bfloat16, device=cuda) for _ in range(2))
     up = torch.empty(B, Q, H, W, device=cuda)
-    _call("odise_upsample_sigmoid_split_f32", m.data_ptr(), hi.data_ptr(), lo.data_ptr(), up.data_ptr(), B, Q, Qp, hs,
-          ws, H, W, _geom(geom))
-    from odise_b200 import lib
+    lib._launch("odise_upsample_sigmoid_split_f32", m, hi, lo, up, B, Q, Qp, hs, ws, H, W, _geom(geom))
     L = lib.load()
     pan = torch.empty(B, H, W, dtype=torch.int32, device=cuda)
     seg_info = torch.zeros(B, Q, 3, dtype=torch.int32, device=cuda)
     nseg = torch.empty(B, dtype=torch.int32, device=cuda)
     pws = torch.empty(int(L.odise_panoptic_ws_bytes(B, Q, H, W)), dtype=torch.uint8, device=cuda)
-    _call("odise_panoptic_inference_f32", m.data_ptr(), scores.data_ptr(), labels.data_ptr(), keep.data_ptr(),
-          it.data_ptr(), pan.data_ptr(), seg_info.data_ptr(), nseg.data_ptr(), pws.data_ptr(), B, Q, K, hs, ws, H, W, 0.8,
-          _geom(geom))
+    lib._launch("odise_panoptic_inference_f32", m, scores, labels, keep, it, pan, seg_info, nseg, pws, B, Q, K, hs, ws, H,
+                W, 0.8, _geom(geom))
     topk = 100
     isc = torch.empty(B, topk, device=cuda)
     icl, iq, iok = (torch.empty(B, topk, dtype=torch.int32, device=cuda) for _ in range(3))
     qm = torch.empty(B, Q, H, W, dtype=torch.uint8, device=cuda)
     iws = torch.empty(int(L.odise_instance_ws_bytes(B, Q, H, W)), dtype=torch.uint8, device=cuda)
-    _call("odise_instance_inference_f32", probs.data_ptr(), m.data_ptr(), it.data_ptr(), isc.data_ptr(), icl.data_ptr(),
-          iq.data_ptr(), iok.data_ptr(), qm.data_ptr(), iws.data_ptr(), B, Q, K, topk, hs, ws, H, W, _geom(geom))
+    lib._launch("odise_instance_inference_f32", probs, m, it, isc, icl, iq, iok, qm, iws, B, Q, K, topk, hs, ws, H, W,
+                _geom(geom))
     torch.cuda.synchronize()
     out = dict(panoptic_seg=pan, seg_info=seg_info, n_segments=nseg, scores=scores.view(B, Q), labels=labels.view(B, Q),
                keep=keep.view(B, Q), instances=dict(scores=isc, pred_classes=icl, query_index=iq, valid=iok,

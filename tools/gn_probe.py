@@ -6,7 +6,7 @@ import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
 from odise_b200 import lib, ops  # noqa: E402
-from odise_b200.lib import Planes, _check, _ptr, _stream, load  # noqa: E402
+from odise_b200.lib import Planes  # noqa: E402
 
 dev = torch.device("cuda")
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -30,14 +30,11 @@ for (B, HW, C) in [(16, 262144, 128), (16, 65536, 256), (16, 16384, 512), (16, 4
                    (16, 1024, 1280), (16, 4096, 960), (4, 65536, 256)]:
     x = torch.randn(B * HW, C, device=dev)
     ga, be = torch.randn(C, device=dev), torch.randn(C, device=dev)
-    mean = torch.empty(B * 32, device=dev)
-    rstd = torch.empty(B * 32, device=dev)
-    t_stats = timeit(lambda: ops._gn_stats(load(), x, C, 0, mean, rstd, B, HW, C, 32, 1e-5))
+    mean, rstd = ops._gn_stats(x, C, 0, B, HW, C, 32, 1e-5, None)
+    t_stats = timeit(lambda: ops._gn_stats(x, C, 0, B, HW, C, 32, 1e-5, None))
     p = Planes.empty(B * HW, C, dev)
-    L = load()
-    t_apply = timeit(lambda: _check(L.odise_groupnorm_apply_f32(_ptr(x), C, _ptr(mean), _ptr(rstd), _ptr(ga), _ptr(be), 2,
-                                                               None, 0, _ptr(p.hi), _ptr(p.lo), p.ld, B, HW, C, 32,
-                                                               _stream()), "apply"))
+    t_apply = timeit(lambda: lib._launch("odise_groupnorm_apply_f32", x, C, mean, rstd, ga, be, 2, None, 0, p.hi, p.lo,
+                                         p.ld, B, HW, C, 32))
     n = B * HW * C
     print(f"B={B} HW={HW} C={C}: stats {t_stats*1000:8.1f} us {4*n/t_stats/1e6:7.0f} GB/s | apply {t_apply*1000:8.1f} us "
           f"{8*n/t_apply/1e6:7.0f} GB/s", flush=True)

@@ -39,7 +39,7 @@ def main():
     eng._gemm(e_silu, "emb_all", "emb_all.b", out=emb_all)
     cpad = torch.zeros(B, 80, 768, device=dev)
     cpad[:, :77] = ctx.to(dev)
-    ctxp = ops.split(cpad.view(B * 80, 768), lo=eng.lo)
+    ctxp = lib.split(cpad.view(B * 80, 768), lo=eng.lo)
 
     def nhwc(x):
         return x.permute(0, 2, 3, 1).reshape(-1, x.shape[1]).contiguous().to(dev)
