@@ -495,10 +495,19 @@ int odise_masked_xattn_backward_bf16(const void* q, const void* k, const void* v
  *   fixed point, so bit-reproducible; rounded once from the fixed-point sum.
  * odise_mask_point_sample_*: out [N, P] float32 = the samples of maps [N, H, W] (_u8: bytes) at points [N, P, 2],
  *   as the kernels above take them: detectron2's point_sample on the device.
+ * odise_mask_assign_f32: scipy.optimize.linear_sum_assignment of every [Q, T_b] block of cost [L, B, Q, Tmax]
+ *   float32 (columns t >= T_b not read), in fp64 and with scipy's shortest-augmenting-path steps, so the indices are
+ *   scipy's, ties included.  tgt_counts: T_b of each image in HOST memory (T_b <= Tmax).  tables int64 receives, set
+ *   after set, pairs [N, 3] = (image, query, global target index) ordered by image then query, pair_of [B*Q] and
+ *   tg_of [B*Q] (each query's pair / global target, -1 if unmatched), N = sum_b min(Q, T_b); every element is written.
+ *   status [L, B] int32: 0 solved, 1 a NaN or -inf cost, 2 infeasible (scipy raises on both); a failed problem gets
+ *   query r <-> target r for r < min(Q, T_b).  B <= ODISE_MASK_MAX_IMAGES and Q, Tmax <= ODISE_MASK_MAX_ASSIGN
+ *   (ODISE_ERR_UNSUPPORTED otherwise); cost may be null when Tmax = 0.
  * Every result is reduced in a fixed order.  No host synchronisation and no allocation. */
 #define ODISE_MASK_MAX_IMAGES 256
 #define ODISE_MASK_MAX_CANDIDATES 53248
 #define ODISE_MASK_MAX_POINTS 32768
+#define ODISE_MASK_MAX_ASSIGN 1024      /* max(Q, T_b) the solver takes */
 long long odise_mask_loss_workspace_bytes(int N, int P);
 int odise_mask_cost_f32(const void* pred, const float* prob, const long long* labels, const uint8_t* tgt,
                         const float* points, const int* tgt_counts, float* cost, int B, int Q, int H, int W, int K1,
@@ -517,6 +526,8 @@ int odise_mask_point_sample_bf16(const void* maps, const float* points, float* o
                                  void* stream);
 int odise_mask_point_sample_u8(const void* maps, const float* points, float* out, int N, int H, int W, int P,
                                void* stream);
+int odise_mask_assign_f32(const float* cost, const int* tgt_counts, long long* tables, int* status, int L, int B, int Q,
+                          int Tmax, void* stream);
 int odise_mask_loss_forward_f32(const void* pred, const uint8_t* tgt, const long long* pairs, const float* cand,
                                 const float* rnd, void* workspace, float* losses, int B, int Q, int H, int W, int Hg,
                                 int Wg, int N, int P, int S, int k, float num_masks, void* stream);

@@ -20,6 +20,12 @@ runs the losses of every set.  num_masks keeps the reference's all_reduce and .i
 initialised (and is computed on the host otherwise), so a forward makes at most 2 synchronising calls.  Any other matcher
 object is called once per set, as the reference does.
 
+With SetCriterion.match_on_device = True, every set on the fused path and max(Q, T_b) <= lib.MASK_MAX_ASSIGN, the
+assignment runs on the device instead (lib.mask_assign: scipy's algorithm, fp64, scipy's indices ties included) and,
+under torch.distributed, num_masks stays the all-reduced device tensor: forward and backward make no synchronising call.
+Where the reference raises ValueError (a NaN or -inf cost, an infeasible problem) this path cannot, as raising needs a
+synchronisation: SetCriterion.match_status [L, B] int32 holds 0, 1 (NaN / -inf) or 2 (infeasible) per (set, image).
+
 The fused path (odise_mask_* kernels) runs a set when its tensors are on CUDA, pred_masks is float32 / float16 /
 bfloat16 [B, Q, H, W], every target's "masks" is bool or uint8 of one [Hg, Wg] on that device, and the point counts are
 within the kernels' limits (lib.MASK_MAX_*).  The target masks are read as bytes: no float copy of a target exists.  The
@@ -253,6 +259,11 @@ class SetCriterion(nn.Module):
         self.oversample_ratio = oversample_ratio
         self.importance_sample_ratio = importance_sample_ratio
         self.use_fused = True
+        # match on the device (lib.mask_assign) when every set is fused: no synchronisation, and invalid costs are
+        # reported in match_status [L, B] (1: NaN or -inf, 2: infeasible) instead of raising ValueError; match_status is
+        # None after a forward that matched with scipy
+        self.match_on_device = False
+        self.match_status = None
 
     # ---- the composed path (the reference's algorithm; CPU indices) ----
 
@@ -327,8 +338,12 @@ class SetCriterion(nn.Module):
         cand, rnd = points()
         if rnd is None:
             rnd = cand.new_empty(cand.shape[0], 0, 2)
+        # a num_masks device tensor divides the sums outside the op, which takes num_masks as a host float
+        on_device = torch.is_tensor(num_masks)
         losses = MaskLossFunction.apply(outputs["pred_masks"].contiguous(), tg.bytes(), tab["pairs"], tab["pair_of"],
-                                        cand, rnd, num_masks, self.num_points, k)
+                                        cand, rnd, 1.0 if on_device else num_masks, self.num_points, k)
+        if on_device:
+            losses = losses / num_masks
         return {"loss_mask": losses[0], "loss_dice": losses[1]}
 
     @staticmethod
@@ -353,27 +368,35 @@ class SetCriterion(nn.Module):
             parts += [pairs.reshape(-1), pair_of, tg_of]
             shapes.append(n)
         host = torch.from_numpy(np.concatenate(parts) if parts else np.zeros(0, np.int64))
-        dev = host.pin_memory().to(device, non_blocking=True)
+        return SetCriterion._split_tables(host.pin_memory().to(device, non_blocking=True), shapes, B, Q)
+
+    @staticmethod
+    def _split_tables(buf, shapes, B, Q):
+        """the per-set views of one int64 table buffer laid out as _tables and lib.mask_assign write it: per set (n
+        pairs) pairs [n, 3], then pair_of [B*Q], then tg_of [B*Q]"""
         out, o = [], 0
         for n in shapes:
-            tab = {"pairs": dev[o:o + 3 * n].view(n, 3)}
+            tab = {"pairs": buf[o:o + 3 * n].view(n, 3)}
             o += 3 * n
-            tab["pair_of"] = dev[o:o + B * Q]
-            tab["tg_of"] = dev[o + B * Q:o + 2 * B * Q]
+            tab["pair_of"] = buf[o:o + B * Q]
+            tab["tg_of"] = buf[o + B * Q:o + 2 * B * Q]
             o += 2 * B * Q
             out.append(tab)
         return out
 
     # ---- forward ----
 
-    def _num_masks(self, targets, device):
+    def _num_masks(self, targets, device, keep_on_device=False):
+        """the reference's num_masks as a float; keep_on_device: under torch.distributed, the all-reduced [1] device
+        tensor itself, without the .item() synchronisation"""
         n = sum(len(t["labels"]) for t in targets)
         if torch.distributed.is_available() and torch.distributed.is_initialized():
             num_masks = torch.as_tensor([n], dtype=torch.float)
             num_masks = num_masks.pin_memory().to(device, non_blocking=True) if device.type == "cuda" else \
                 num_masks.to(device)
             torch.distributed.all_reduce(num_masks)
-            return torch.clamp(num_masks / torch.distributed.get_world_size(), min=1).item()
+            num_masks = torch.clamp(num_masks / torch.distributed.get_world_size(), min=1)
+            return num_masks if keep_on_device else num_masks.item()
         return torch.clamp(torch.as_tensor([n], dtype=torch.float), min=1).item()
 
     def forward(self, outputs, targets):
@@ -419,15 +442,20 @@ class SetCriterion(nn.Module):
             else:
                 draws.append((mp, self._draw_loss(N, dev)))
         rng_end = torch.cuda.get_rng_state(device) if any(fused) and masks else None
-        num_masks = self._num_masks(targets, device)
+        on_device = self.match_on_device and all(fused) and max(Q, tg.Tmax) <= lib.MASK_MAX_ASSIGN
+        num_masks = self._num_masks(targets, device, keep_on_device=on_device)
         C = torch.empty(len(sets), B, Q, tg.Tmax, dtype=torch.float32, device=sets[0]["pred_masks"].device)
         for l, out in enumerate(sets):
             m._costs(out, tg, draws[l][0], C[l], fused=self.use_fused)
-        indices = _assign(C, tg.counts)
-        tabs = {}
-        if any(fused):
-            sel = [l for l, f in enumerate(fused) if f]
-            tabs = dict(zip(sel, self._tables([indices[l] for l in sel], tg.counts, Q, sets[0]["pred_masks"].device)))
+        if on_device:
+            buf, self.match_status = lib.mask_assign(C, tg.counts)
+            indices, tabs = None, dict(enumerate(self._split_tables(buf, [N] * len(sets), B, Q)))
+        else:
+            indices, tabs, self.match_status = _assign(C, tg.counts), {}, None
+            if any(fused):
+                sel = [l for l, f in enumerate(fused) if f]
+                tabs = dict(zip(sel, self._tables([indices[l] for l in sel], tg.counts, Q,
+                                                  sets[0]["pred_masks"].device)))
         losses = {}
         for l, (out, sfx) in enumerate(zip(sets, names)):
             for loss in self.losses:

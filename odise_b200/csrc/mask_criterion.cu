@@ -25,6 +25,14 @@
 // gradients of a matched query are summed into the map with the bilinear corner weights in int64 fixed point in shared
 // memory (scale 2^(62 - e), P * max|g| < 2^e, computed in the CTA): integer sums do not depend on the order of the
 // atomics, so the gradient is bit-reproducible without any switch.
+//
+// Assignment (mc_assign_kernel, one warp per (set, image) problem): scipy.optimize.linear_sum_assignment's shortest
+// augmenting path (scipy/optimize/rectangular_lsap), step for step and in the same fp64 arithmetic, so the matched pairs
+// are scipy's for every input, ties included.  A [Q, T] block with T < Q is solved transposed (rows = targets), as
+// scipy does.  The sequential column scan's choice (the smallest reduced cost; among equal ones the last unassigned
+// column in `remaining` order, else the first) is the warp-wide minimum of the key (cost, rank) with rank = MAX - 1 - it
+// for an unassigned column and MAX + it for an assigned one.  Every update is an add or a subtract in scipy's operand
+// order: nothing can be contracted into an FMA.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -414,6 +422,163 @@ __global__ void mc_point_sample_kernel(const T* __restrict__ maps, const float* 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// assignment
+
+constexpr int MA_MAX = ODISE_MASK_MAX_ASSIGN;
+constexpr int MA_STAGE_SMEM = 64 * 1024;   // the cost block is staged in shared memory when the CTA stays below this
+
+// shared bytes of the solver's state for max(Q, T) <= M (M a multiple of 8, so every array stays 16-byte aligned):
+// u, v, spc fp64, path, row4col, col4row, remaining int16, SR, SC bytes
+__host__ __device__ __forceinline__ int ma_state_bytes(int M) { return M * (3 * 8 + 4 * 2 + 2); }
+
+__global__ void __launch_bounds__(32) mc_assign_kernel(const float* __restrict__ cost, McCounts cnt,
+                                                       long long* __restrict__ tables, int* __restrict__ status, int B,
+                                                       int Q, int Tmax, int M, int N, int staged) {
+  extern __shared__ __align__(16) unsigned char ma_smem[];
+  double* u = reinterpret_cast<double*>(ma_smem);
+  double* v = u + M;
+  double* spc = v + M;
+  short* path = reinterpret_cast<short*>(spc + M);
+  short* row4col = path + M;
+  short* col4row = row4col + M;
+  short* rem = col4row + M;
+  unsigned char* SR = reinterpret_cast<unsigned char*>(rem + M);
+  unsigned char* SC = SR + M;
+  float* stage = reinterpret_cast<float*>(ma_smem + ma_state_bytes(M));
+  const int l = blockIdx.x / B, b = blockIdx.x % B, lane = threadIdx.x;
+  const int T = cnt.n[b];
+  const bool tr = T < Q;
+  const int nr = tr ? T : Q, nc = tr ? Q : T;
+  const float* blk = cost + ((long long)l * B + b) * Q * Tmax;
+
+  // scipy's "invalid numeric entries" test (NaN or -inf anywhere), while the block is staged as [nr, nc]
+  bool bad = false;
+  for (int e = lane; e < Q * T; e += 32) {
+    const int q = e / T, t = e % T;
+    const float x = __ldg(blk + (long long)q * Tmax + t);
+    bad |= x != x || x == -INFINITY;
+    if (staged) stage[tr ? t * nc + q : q * nc + t] = x;
+  }
+  // c(i, j) = c[i * si + j * sj]
+  const float* c = staged ? stage : blk;
+  const long long si = staged ? nc : (tr ? 1 : Tmax), sj = staged ? 1 : (tr ? Tmax : 1);
+  int st = __any_sync(0xffffffffu, bad) ? 1 : 0;
+  for (int j = lane; j < nc; j += 32) {
+    v[j] = 0.0;
+    row4col[j] = -1;
+  }
+  for (int i = lane; i < nr; i += 32) {
+    u[i] = 0.0;
+    col4row[i] = -1;
+  }
+  __syncwarp();
+
+  for (int cur = 0; cur < nr && st == 0; ++cur) {
+    for (int j = lane; j < nc; j += 32) {
+      spc[j] = INFINITY;
+      SC[j] = 0;
+      rem[j] = (short)(nc - 1 - j);
+    }
+    for (int i = lane; i < nr; i += 32) SR[i] = 0;
+    __syncwarp();
+    int i = cur, nrem = nc, sink = -1;
+    double minVal = 0.0;
+    while (sink < 0) {
+      if (lane == 0) SR[i] = 1;
+      const double ui = u[i];
+      const float* ci = c + i * si;
+      double bv = INFINITY;
+      int bk = 2 * MA_MAX;
+      for (int it = lane; it < nrem; it += 32) {
+        const int j = rem[it];
+        const double r = minVal + (double)ci[j * sj] - ui - v[j];
+        double s = spc[j];
+        if (r < s) {
+          path[j] = (short)i;
+          spc[j] = r;
+          s = r;
+        }
+        const int k = row4col[j] < 0 ? MA_MAX - 1 - it : MA_MAX + it;
+        if (s < bv || (s == bv && k < bk)) {
+          bv = s;
+          bk = k;
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
+        if (ov < bv || (ov == bv && ok < bk)) {
+          bv = ov;
+          bk = ok;
+        }
+      }
+      if (bv == INFINITY) {   // scipy's "cost matrix is infeasible"
+        st = 2;
+        break;
+      }
+      minVal = bv;
+      const int idx = bk < MA_MAX ? MA_MAX - 1 - bk : bk - MA_MAX;
+      const int j = rem[idx], owner = row4col[j];
+      __syncwarp();
+      if (lane == 0) {
+        SC[j] = 1;
+        rem[idx] = rem[nrem - 1];
+      }
+      --nrem;
+      if (owner < 0) sink = j;
+      else i = owner;
+      __syncwarp();
+    }
+    if (st) break;
+    if (lane == 0) u[cur] += minVal;
+    for (int r = lane; r < nr; r += 32)
+      if (SR[r] && r != cur) u[r] += minVal - spc[col4row[r]];
+    for (int j = lane; j < nc; j += 32)
+      if (SC[j]) v[j] -= minVal - spc[j];
+    __syncwarp();
+    if (lane == 0) {
+      for (int j = sink;;) {
+        const int r = path[j];
+        row4col[j] = (short)r;
+        const int nj = col4row[r];
+        col4row[r] = (short)j;
+        j = nj;
+        if (r == cur) break;
+      }
+    }
+    __syncwarp();
+  }
+
+  // the set's tables: pairs [N, 3], pair_of [B*Q], tg_of [B*Q]; pairs by image, then by query ascending.  A problem
+  // that failed gets query r <-> target r for r < min(Q, T), in range for the loss kernels.
+  long long* pairs = tables + (long long)l * (3ll * N + 2ll * B * Q);
+  long long* pair_of = pairs + 3ll * N + (long long)b * Q;
+  long long* tg_of = pair_of + (long long)B * Q;
+  int n0 = 0;
+  for (int k = 0; k < b; ++k) n0 += min(Q, cnt.n[k]);
+  const long long toff = cnt.off[b];
+  for (int q0 = 0; q0 < Q; q0 += 32) {
+    const int q = q0 + lane;
+    int t = -1;
+    if (q < Q) t = st ? (q < min(Q, T) ? q : -1) : tr ? row4col[q] : col4row[q];
+    const unsigned hit = __ballot_sync(0xffffffffu, t >= 0);
+    const long long n = n0 + __popc(hit & ((1u << lane) - 1u));
+    if (q < Q) {
+      pair_of[q] = t >= 0 ? n : -1;
+      tg_of[q] = t >= 0 ? toff + t : -1;
+      if (t >= 0) {
+        pairs[3 * n] = b;
+        pairs[3 * n + 1] = q;
+        pairs[3 * n + 2] = toff + t;
+      }
+    }
+    n0 += __popc(hit);
+  }
+  if (lane == 0) status[(long long)l * B + b] = st;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // host side
 
 int mc_check_maps(int B, int Q, int H, int W, int Hg, int Wg) {
@@ -523,6 +688,32 @@ int mc_point_sample(const void* maps, const float* points, float* out, int N, in
   return (int)cudaGetLastError();
 }
 
+int mc_assign(const float* cost, const int* tgt_counts, long long* tables, int* status, int L, int B, int Q, int Tmax,
+              void* stream) {
+  if (!tgt_counts || !tables || !status || L <= 0 || B <= 0 || Q <= 0 || Tmax < 0 || (!cost && Tmax > 0))
+    return ODISE_ERR_ARG;
+  if (B > ODISE_MASK_MAX_IMAGES || Q > MA_MAX || Tmax > MA_MAX) return ODISE_ERR_UNSUPPORTED;
+  if ((long long)L * B > 0x7fffffffll) return ODISE_ERR_UNSUPPORTED;
+  McCounts cnt;
+  int off = 0, N = 0;
+  for (int b = 0; b < B; ++b) {
+    if (tgt_counts[b] < 0 || tgt_counts[b] > Tmax) return ODISE_ERR_ARG;
+    cnt.n[b] = tgt_counts[b];
+    cnt.off[b] = off;
+    off += tgt_counts[b];
+    N += min(Q, tgt_counts[b]);
+  }
+  const int M = (max(Q, Tmax) + 7) / 8 * 8;
+  int smem = ma_state_bytes(M);
+  const int staged = smem + Q * Tmax * 4 <= MA_STAGE_SMEM;
+  if (staged) smem += Q * Tmax * 4;
+  cudaError_t e = cudaFuncSetAttribute(mc_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return (int)e;
+  mc_assign_kernel<<<L * B, 32, smem, (cudaStream_t)stream>>>(cost, cnt, tables, status, B, Q, Tmax, M, N, staged);
+  count_launch(1);
+  return (int)cudaGetLastError();
+}
+
 }  // namespace
 }  // namespace ob
 
@@ -566,6 +757,11 @@ OB_MC_ENTRIES(bf16, __nv_bfloat16)
 int odise_mask_point_sample_u8(const void* maps, const float* points, float* out, int N, int H, int W, int P,
                                void* stream) {
   return ob::mc_point_sample<uint8_t>(maps, points, out, N, H, W, P, stream);
+}
+
+int odise_mask_assign_f32(const float* cost, const int* tgt_counts, long long* tables, int* status, int L, int B, int Q,
+                          int Tmax, void* stream) {
+  return ob::mc_assign(cost, tgt_counts, tables, status, L, B, Q, Tmax, stream);
 }
 
 }  // extern "C"

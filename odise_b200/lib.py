@@ -677,6 +677,7 @@ def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
 
 
 MASK_MAX_IMAGES, MASK_MAX_CANDIDATES, MASK_MAX_POINTS = 256, 53248, 32768    # ODISE_MASK_MAX_* of the header
+MASK_MAX_ASSIGN = 1024                                                          # ODISE_MASK_MAX_ASSIGN
 _MASK_BYTES = (torch.bool, torch.uint8)
 
 
@@ -743,6 +744,31 @@ def mask_cost(pred, prob, labels, tgt, points, counts, w_class, w_mask, w_dice, 
     _launch("odise_mask_cost_" + sfx, pred, prob, labels, _u8(tgt), points, cnt, out, B, Q, H, W, K1, Hg, Wg, Tmax, P,
             float(w_class), float(w_mask), float(w_dice))
     return out
+
+
+def mask_assign(cost, counts):
+    """scipy.optimize.linear_sum_assignment of every [Q, counts[b]] block of cost [L, B, Q, Tmax] float32 on the device
+    (odise_mask_assign_f32), scipy's indices for every input, ties included; counts: a Python list ->
+    (tables, status).  tables int64 holds, set after set, pairs [N, 3] (image, query, global target) by image then
+    query, pair_of [B*Q] and tg_of [B*Q] (-1 if unmatched), N = sum_b min(Q, counts[b]); status [L, B] int32 is
+    0 (solved), 1 (a NaN or -inf cost) or 2 (infeasible), where scipy raises.  No synchronisation, CUDA-graph
+    capturable.  OdiseError on CPU, non-contiguous or wrongly typed costs, counts that disagree, B > MASK_MAX_IMAGES
+    and Q or Tmax > MASK_MAX_ASSIGN."""
+    _tensor(cost, "cost", torch.float32)
+    if cost.dim() != 4:
+        raise OdiseError(f"cost must be [L, B, Q, Tmax], got {tuple(cost.shape)}")
+    L, B, Q, Tmax = cost.shape
+    counts = [int(c) for c in counts]
+    if min(L, B, Q) <= 0 or len(counts) != B or not all(0 <= c <= Tmax for c in counts):
+        raise OdiseError(f"target counts {counts} do not match cost {tuple(cost.shape)}")
+    if B > MASK_MAX_IMAGES or max(Q, Tmax) > MASK_MAX_ASSIGN:
+        raise OdiseError(f"mask assign: at most {MASK_MAX_IMAGES} images and {MASK_MAX_ASSIGN} queries and targets, "
+                         f"got cost {tuple(cost.shape)}")
+    N = sum(min(Q, c) for c in counts)
+    tables = torch.empty(L * (3 * N + 2 * B * Q), dtype=torch.int64, device=cost.device)
+    status = torch.empty(L, B, dtype=torch.int32, device=cost.device)
+    _launch("odise_mask_assign_f32", cost, (ctypes.c_int * B)(*counts), tables, status, L, B, Q, Tmax)
+    return tables, status
 
 
 def _mask_loss_shapes(pred, tgt, pairs, num_points):
