@@ -245,7 +245,8 @@ typedef struct odise_gemm_desc {
   float* out_f32; long long ld_out; long long out_batch_stride;
   void* out_hi; void* out_lo; long long ld_out_bf16; long long out_bf16_batch_stride;
   int split_k; void* workspace; long long workspace_bytes;
-  int force_bn;                      /* 0 = heuristic; 64/128/160/256 */
+  int force_bn;                      /* 0 = autotuned / cost model; 64/128/160/256 = that output-tile width, bypassing
+                                        the autotune and its per-shape cache (nmma 2 runs 160 and 256 as 128) */
   const float* bias_m;               /* [M] per-row bias or NULL (transposed-output projections) */
   int conv_mode;                     /* conv3x3: 0 = stride 1 pad 1; 1 = stride 2 pad (1,1) (ldm Downsample);
                                         2 = stride 2 pad (0,1) (ldm VAE Downsample). conv_H/W are INPUT dims,

@@ -133,29 +133,28 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-// epilogue for 4 consecutive columns [n, n+4) of row m (n % 4 == 0); `valid` = how many of them exist (N tail)
+// epilogue for 4 consecutive columns [n, n+4) of row m (n % 4 == 0); `valid` = how many of them exist (N tail).
+// alpha, bias and bias_m take the interior path's single fmaf with the same addend (bias + bias_m in its EPI = 1
+// instantiation, the bias alone in EPI = 0), so a column rounds the same whether a tile width puts it in an interior or
+// an edge tile: every width gives the same bits, signed zeros included.
 __device__ __forceinline__ void epilogue_quad(const GemmParams& p, int z, int m, int n, int valid, float4 a4,
                                               float* final_vals = nullptr) {
   float acc[4] = {a4.x, a4.y, a4.z, a4.w};
   const bool vec = (valid == 4) && p.vec_ok;
-  if (p.alpha != 1.f) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[j] *= p.alpha;
-  }
+  float b[4] = {0.f, 0.f, 0.f, 0.f};
   if (p.bias) {
     if (vec) {
-      const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-      acc[0] += b.x; acc[1] += b.y; acc[2] += b.z; acc[3] += b.w;
+      const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n));
+      b[0] = b4.x; b[1] = b4.y; b[2] = b4.z; b[3] = b4.w;
     } else {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) if (j < valid) acc[j] += __ldg(p.bias + n + j);
+      for (int j = 0; j < 4; ++j) if (j < valid) b[j] = __ldg(p.bias + n + j);
     }
   }
-  if (p.bias_m) {
-    const float bm = __ldg(p.bias_m + m);
+  const bool extra = p.bias_m || p.rowbias || p.res;   // the host's epi == 1
+  const float bm = p.bias_m ? __ldg(p.bias_m + m) : 0.f;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[j] += bm;
-  }
+  for (int j = 0; j < 4; ++j) acc[j] = fmaf(acc[j], p.alpha, extra ? b[j] + bm : b[j]);
   if (p.rowbias) {
     const float* rb = p.rowbias + (long long)(((long long)z * p.M + m) / p.rows_per_group) * p.rowbias_ld + n;
     if (vec) {
@@ -854,9 +853,11 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
     return r;
   };
 
-  // ---- tile width: a per-shape autotune (every candidate is the same arithmetic in the same k order -> bit-identical
-  // results, so the choice is free) with the cost model pick_tile() as the fallback under stream capture.
-  // ODISE_GEMM_AUTOTUNE=0: cost model only.
+  // ---- tile width: a per-shape autotune (every candidate is the same arithmetic in the same k order, and edge tiles
+  // round the epilogue like interior ones -> bit-identical results, so the choice is free; tests/test_gpu_gemm_widths.py
+  // checks every width against the autotuned one) with the cost model pick_tile() as the fallback under stream capture.
+  // ODISE_GEMM_AUTOTUNE=0: cost model only.  A valid force_bn overrides both: it skips the autotune and its cache
+  // (F16Q8, nmma 2, runs a forced 160 or 256 as 128).
   int BN;
   {
     static const bool tune = !(getenv("ODISE_GEMM_AUTOTUNE") && atoi(getenv("ODISE_GEMM_AUTOTUNE")) == 0);
@@ -873,10 +874,11 @@ extern "C" int odise_gemm_bf16(const odise_gemm_desc* d, void* stream_v) {
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(stream, &cap);
     std::lock_guard<std::mutex> lk(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) {
+    if (fbn) {
+      // the forced width as pick_tile() mapped it: no cache lookup, no trial runs, no cache entry
+    } else if (auto it = cache.find(key); it != cache.end()) {
       BN = it->second;
-    } else if (tune && !fbn && !g_prof_on && cap == cudaStreamCaptureStatusNone &&
+    } else if (tune && !g_prof_on && cap == cudaStreamCaptureStatusNone &&
                !(d->residual && (const void*)d->residual == (const void*)d->out_f32)) {
       // candidates from wide to narrow (64 only for narrow outputs)
       const int cands[4] = {256, 160, 128, 64};
