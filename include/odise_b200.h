@@ -471,6 +471,39 @@ int odise_masked_xattn_backward_bf16(const void* q, const void* k, const void* v
                                      void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * UNet attention for training (ldm's CrossAttention in the SD-v1 UNet, self- and cross-attention), forward and backward
+ * of the attention core
+ *   out[b, i, h, :] = softmax_j(s * q[b, i, h, :] . k[b, j, h, :]) v[b, j, h, :],  s = 1/sqrt(D)
+ * on the batch-first layouts of to_q / to_k / to_v: q and out [B, Tq, H*D], k and v [B, Tk, H*D], heads interleaved in
+ * the last dimension, contiguous.  D = 40, 80 or 160 (ODISE_ERR_UNSUPPORTED otherwise); B, H, Tq, Tk >= 1 and
+ * B*H <= 65535 (ODISE_ERR_ARG otherwise).  _f32 / _f16 / _bf16: q, k, v, out, grad_out and the gradients in float,
+ * __half or __nv_bfloat16 (one type).  Tensor cores with fp32 accumulation: 16-bit operands one MMA per product, with
+ * the probabilities and their gradients rounded to the storage type before they enter a product; float operands split
+ * into three TF32 products (about 2^-22 relative error per product).  lse [B*H, Tq] float32 = the log-sum-exp of each
+ * row's scaled scores, the only thing the backward needs beyond the inputs and out.  The backward's workspace
+ * (odise_unet_attn_workspace_bytes(B, H, D, Tq, Tk) bytes, 16-byte aligned, any content) holds delta = rowsum(dO o O)
+ * and, where the keys alone give too few blocks, fp32 partial dK / dV sums over query chunks whose number depends on the
+ * shape only, added in chunk order: grad_q, grad_k and grad_v are bit-reproducible (no atomics).  Pointers to the
+ * storage-type tensors must be 16-byte (float) or 8-byte (16-bit) aligned (ODISE_ERR_ALIGN).  No host synchronisation
+ * and no allocation (CUDA-graph capturable).  workspace_bytes returns 0 for shapes the entry points refuse. */
+long long odise_unet_attn_workspace_bytes(int B, int H, int D, int Tq, int Tk);
+int odise_unet_attn_forward_f32(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int D,
+                                int Tq, int Tk, void* stream);
+int odise_unet_attn_forward_f16(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int D,
+                                int Tq, int Tk, void* stream);
+int odise_unet_attn_forward_bf16(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H,
+                                 int D, int Tq, int Tk, void* stream);
+int odise_unet_attn_backward_f32(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                                 const void* grad_out, void* grad_q, void* grad_k, void* grad_v, int B, int H, int D,
+                                 int Tq, int Tk, void* workspace, void* stream);
+int odise_unet_attn_backward_f16(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                                 const void* grad_out, void* grad_q, void* grad_k, void* grad_v, int B, int H, int D,
+                                 int Tq, int Tk, void* workspace, void* stream);
+int odise_unet_attn_backward_bf16(const void* q, const void* k, const void* v, const void* out, const float* lse,
+                                  const void* grad_out, void* grad_q, void* grad_k, void* grad_v, int B, int H, int D,
+                                  int Tq, int Tk, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Mask2Former SetCriterion for training (matcher.py:15-156, criterion.py:21-197): Hungarian matching costs and the
  * point-sampled mask losses with their backward.  pred [B, Q, H, W] in float, __half or __nv_bfloat16 (_f32 / _f16 /
  * _bf16); target masks tgt [sum T, Hg, Wg] bytes (0 / 1: a torch bool or uint8 tensor), image b's targets first-to-last

@@ -499,6 +499,7 @@ def msda_backward(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     return [grad_value, grad_loc, grad_attn]
 
 
+ODISE_ERR_ARG, ODISE_ERR_ALIGN, ODISE_ERR_WORKSPACE = 10001, 10002, 10005     # the header's ODISE_ERR_*
 ODISE_ERR_UNSUPPORTED = 10006
 
 
@@ -673,6 +674,63 @@ def masked_xattn_backward(q, k, v, mask, out, lse, grad_out, heads):
     gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
     _launch("odise_masked_xattn_backward_" + _SFX[q.dtype], q, k, v, mask, stride, out, lse, grad_out, gq, gk, gv, B,
             heads, 32, Q, S, workspace=lambda dll: dll.odise_masked_xattn_workspace_bytes(B, heads, Q, S))
+    return gq, gk, gv
+
+
+UNET_ATTN_HEAD_DIMS = (40, 80, 160)     # SD-v1's 320 / 640 / 1280 channels over 8 heads
+
+
+def unet_attn_supported(B, heads, dim_head, Tq, Tk):
+    """whether the UNet attention kernels take B images of `heads` heads of dim_head channels, Tq queries and Tk keys:
+    a head dim of UNET_ATTN_HEAD_DIMS, non-empty sequences and at most 65535 (image, head) pairs"""
+    return (dim_head in UNET_ATTN_HEAD_DIMS and min(B, heads, Tq, Tk) >= 1 and B * heads <= 65535
+            and max(Tq, Tk) * B * heads * 160 < 2 ** 40)
+
+
+def _unet_attn_shapes(q, k, v, heads, out=None, lse=None, grad_out=None):
+    """Checks of the UNet attention entry points, without data and without the library: q [B, Tq, heads*D], k and v
+    [B, Tk, heads*D] as to_q / to_k / to_v write them, contiguous CUDA tensors of one dtype of float32 / float16 /
+    bfloat16, unet_attn_supported(B, heads, D, Tq, Tk); for the backward out and grad_out like q and lse [B*heads, Tq]
+    float32.  -> (B, Tq, Tk, D)"""
+    _tensor(q, "q", _FLOATS)
+    if q.dim() != 3 or k.dim() != 3:
+        raise OdiseError(f"q and k: expected 3-D tensors, got {tuple(q.shape)} and {tuple(k.shape)}")
+    B, Tq, E = q.shape
+    Tk = k.shape[1]
+    if heads <= 0 or E % heads:
+        raise OdiseError(f"inner dim {E} is not divisible by heads = {heads}")
+    D = E // heads
+    if not unet_attn_supported(B, heads, D, Tq, Tk):
+        raise OdiseError(f"UNet attention: B = {B}, heads = {heads}, head dim {D}, Tq = {Tq}, Tk = {Tk} not supported "
+                         f"(head dim one of {UNET_ATTN_HEAD_DIMS}, non-empty sequences, B*heads <= 65535)")
+    for t, nm, want in ((k, "k", (B, Tk, E)), (v, "v", (B, Tk, E)), (out, "out", (B, Tq, E)),
+                        (grad_out, "grad_out", (B, Tq, E))):
+        if t is not None:
+            _tensor(t, nm, q.dtype, want)
+    if lse is not None:
+        _tensor(lse, "lse", torch.float32, (B * heads, Tq))
+    return B, Tq, Tk, D
+
+
+def unet_attn_forward(q, k, v, heads):
+    """Attention core of ldm's CrossAttention (odise_unet_attn_forward_f32 / _f16 / _bf16 by q.dtype): q [B, Tq,
+    heads*D], k and v [B, Tk, heads*D], D = 40, 80 or 160 -> (out [B, Tq, heads*D] in q's dtype, lse [B*heads, Tq]
+    float32).  OdiseError on CPU, non-contiguous or mixed-dtype tensors, shapes that disagree and unsupported shapes."""
+    B, Tq, Tk, D = _unet_attn_shapes(q, k, v, heads)
+    out = torch.empty_like(q)
+    lse = torch.empty(B * heads, Tq, dtype=torch.float32, device=q.device)
+    _launch("odise_unet_attn_forward_" + _SFX[q.dtype], q, k, v, out, lse, B, heads, D, Tq, Tk)
+    return out, lse
+
+
+def unet_attn_backward(q, k, v, out, lse, grad_out, heads):
+    """Backward of unet_attn_forward (odise_unet_attn_backward_*) -> (grad_q, grad_k, grad_v) shaped and typed like
+    q / k / v.  grad_out has q's dtype.  Every result is bit-reproducible (fixed-order sums, no atomics).  Errors as
+    unet_attn_forward, and for out / lse / grad_out of the wrong shape or dtype."""
+    B, Tq, Tk, D = _unet_attn_shapes(q, k, v, heads, out=out, lse=lse, grad_out=grad_out)
+    gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    _launch("odise_unet_attn_backward_" + _SFX[q.dtype], q, k, v, out, lse, grad_out, gq, gk, gv, B, heads, D, Tq, Tk,
+            workspace=lambda dll: dll.odise_unet_attn_workspace_bytes(B, heads, D, Tq, Tk))
     return gq, gk, gv
 
 
